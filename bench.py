@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """bench.py -- mpileup reference positions/sec on the BASELINE workloads.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--region-mb M] [--modes a,b,...]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--region-mb M] [--modes a,b,...] [--dump-outputs DIR]
   (N>1: python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...)
 
 ONE JSON line.  Its top-level keys are the headline workload; `modes` holds one sub-record per further
@@ -15,7 +15,7 @@ BASELINE configuration, each with its own value / roofline / cpu_baseline:
                  (bcf_call_glfgen + errmod_cal, bam2bcf.c:65-123)
 
 A "step" is one pass of the hot path over one staged batch; inputs (0.05 GB/Mb) and outputs (0.08 GB/Mb) of a
-step are far larger than the 126 MB L2, so successive steps cannot be served from cache.  With N GPUs every
+step are far larger than the 50 MB L2 of an H100, so successive steps cannot be served from cache.  With N GPUs every
 rank owns its own region (weak scaling, no data-path collective; the one collective is the all_gather of the
 per-region column summaries rank 0 needs to emit shards in genome order, issued once for all timed steps).
 
@@ -28,6 +28,9 @@ cpu_baseline / --impl reference: the CPU oracle (the reference cannot be built h
        DESIGN.md) on the box's host cores -- as many processes as the scheduler affinity AND the cgroup CPU
        quota allow; the per-process and the single-process rates are reported next to the total so that a
        starved box is visible.
+--dump-outputs DIR  after the timed steps, rank 0 writes what a caller received from the last step as DIR/<name>.npy
+       (float32 / float64): the end-to-end loop's mpileup text (seeded 64 KiB slices of it, their offsets, its length) and the
+       coverage sums of the `coverage` mode.  Inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -45,33 +48,17 @@ import numpy as np  # noqa: E402
 METRIC = 'mpileup reference positions/sec'
 UNIT = 'positions/s'
 ALL_MODES = ('mpileup_f_baq', 'depth_a', 'coverage', 'gl_c4')
-# nominal non-fused FP64 rate of a B200: 148 SMs x 64 FP64 lanes x 1.965 GHz (an FMA counts as ONE issue slot here
-# because BAQ must not contract a*b+c); no driver-measured figure exists for this pipe
-FP64_NONFMA_PEAK = 148 * 64 * 1.965e9
+# FP64 lanes per SM on sm_90; the nominal non-fused FP64 rate is SMs x lanes x max SM clock (an FMA counts as ONE issue slot
+# here because BAQ must not contract a*b+c)
+FP64_LANES_PER_SM = 64
+DUMP_SLICES, DUMP_SLICE_BYTES = 128, 65536
 
 
 def peaks():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
         return float(json.load(open(p))['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
-    return 6650.0, 'fallback (B200_PROFILING.md)'
-
-
-def measured_traffic(kernels):
-    """DRAM bytes per launch of the named kernels from the round's ncu capture (profiles/r02_traffic.json, written by
-    tools/ncu_traffic.py) -- only while the kernel sources are the ones the capture was taken from; otherwise None."""
-    p = os.path.join(ROOT, 'profiles', 'r02_traffic.json')
-    try:
-        import hashlib
-        rec = json.load(open(p))
-        h = hashlib.sha256()
-        for s_ in rec['sources']:
-            h.update(open(os.path.join(ROOT, s_), 'rb').read())
-        if h.hexdigest() != rec['sources_sha256']:
-            return None
-        return float(sum(rec['dram_bytes_per_launch'][k] for k in kernels))
-    except Exception:
-        return None
+    return 3350.0, 'data sheet (H100 SXM HBM3: 3.35 TB/s), not measured'
 
 
 def usable_cores():
@@ -292,7 +279,7 @@ def workload_config(args):
     return {'workload': f'BASELINE C2 shape x{args.region_mb:g}: synthetic {args.region_mb:g} Mb region per GPU, 30x depth, 150 bp paired reads, '
                         f'`mpileup -a` (no FASTA -> no BAQ, overlap removal on, -Q13, -d 8000)',
             'region_mb_per_gpu': args.region_mb, 'depth': 30, 'read_len': 150,
-            'l2_policy': 'inputs (0.05 GB/Mb) and outputs (0.08 GB/Mb) per step exceed the 126 MB L2; no explicit flush',
+            'l2_policy': 'inputs (0.05 GB/Mb) and outputs (0.08 GB/Mb) per step exceed the 50 MB L2; no explicit flush',
             'parallelism': f'region-shard x{args.gpus}',
             'modes': 'sub-records: mpileup_f_baq (same window + FASTA, BAQ on), depth_a, coverage (same window), gl_c4 (200x panel with 2000x hotspots)'}
 
@@ -321,6 +308,23 @@ def pin(soa):
     return out
 
 
+def dump_outputs(d, text, cov_sums):
+    """DIR/<name>.npy: seeded 64 KiB slices of the mpileup text (bytes as float32), their offsets and the text length (float64),
+    and the coverage sums (float64) -- well under 64 MB in all"""
+    os.makedirs(d, exist_ok=True)
+    n = len(text)
+    k = min(DUMP_SLICES, max(1, n // DUMP_SLICE_BYTES))
+    span = max(1, n - DUMP_SLICE_BYTES + 1)
+    offs = np.sort(np.random.default_rng(12345).choice(span, size=min(k, span), replace=False))
+    sample = np.concatenate([text[o:o + DUMP_SLICE_BYTES] for o in offs]) if n else np.zeros(0, np.uint8)
+    np.save(os.path.join(d, 'mpileup_text_len.npy'), np.array([n], np.float64))
+    np.save(os.path.join(d, 'mpileup_text_slice_offsets.npy'), offs.astype(np.float64))
+    np.save(os.path.join(d, 'mpileup_text_slices.npy'), sample.astype(np.float32))
+    if cov_sums is not None:
+        names = sorted(cov_sums)
+        np.save(os.path.join(d, 'coverage_sums.npy'), np.array([cov_sums[k_] for k_ in names], np.float64))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--gpus', type=int, default=1)
@@ -332,6 +336,7 @@ def main():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--e2e-handles', type=int, default=4,
                     help='engine handles (one host thread each) used by the end-to-end loop; handles are per-thread objects like the htslib iterators they replace')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the last step\'s outputs as DIR/<name>.npy (see the module docstring)')
     args = ap.parse_args()
     if args.impl == 'reference':
         return reference_arm(args)
@@ -415,7 +420,7 @@ def main():
         return n.value
 
     def run_e2e(k_steps):
-        """k_steps windows through n_h handles; returns bytes of the last window"""
+        """k_steps windows through n_h handles; returns the text of the last window (a view of its host buffer)"""
         res = [0] * n_h
         def worker(j):
             for s_ in range(j, k_steps, n_h):
@@ -424,7 +429,8 @@ def main():
         ths = [_th.Thread(target=worker, args=(j,)) for j in range(n_h)]
         [t.start() for t in ths]; [t.join() for t in ths]
         exchange_summaries()
-        return max(res)
+        last = (k_steps - 1) % n_h
+        return outs[last][:res[last]]
 
     for _ in range(args.warmup):
         run_e2e(n_h); step_device()
@@ -448,7 +454,7 @@ def main():
         # ---- end to end through the C ABI with host buffers
         sync_all()
         t0 = time.perf_counter()
-        run_e2e(args.steps)
+        last_text = run_e2e(args.steps)
         sync_all()
         dt_e2e = time.perf_counter() - t0
     dt = shard.max_over_ranks(dt, dev); dt_e2e = shard.max_over_ranks(dt_e2e, dev)
@@ -457,6 +463,8 @@ def main():
         h.close()
 
     peak, peak_src = peaks()
+    props = torch.cuda.get_device_properties(dev)
+    fp64_peak = props.multi_processor_count * FP64_LANES_PER_SM * clocks['sm_max_mhz'] * 1e6 if clocks['sm_max_mhz'] else None
     line = None
     if rank == 0:
         kms = float(np.mean(kernel_ms))
@@ -466,21 +474,20 @@ def main():
         # gather consumes every read base once and writes every text byte once -> bytes_in + bytes_out; the entry pass reads the
         # staged reads once -> bytes_in (its entry strings are an intermediate, not algorithmic traffic)
         if write_ms >= size_ms:
-            dom, alg, dom_ms, dom_k = 'k_mp_gather (entry strings -> text)', bytes_in + out_len, write_ms, ['k_mp_gather']
+            dom, alg, dom_ms = 'k_mp_gather (entry strings -> text)', bytes_in + out_len, write_ms
         else:
-            dom, alg, dom_ms, dom_k = 'k_mp_entries + k_ss_scan + k_ss_cols (reads -> entry strings, line sizes)', bytes_in, size_ms, ['k_mp_entries', 'k_ss_scan', 'k_ss_cols']
+            dom, alg, dom_ms = 'k_mp_entries + k_ss_scan + k_ss_cols (reads -> entry strings, line sizes)', bytes_in, size_ms
         achieved = alg / (dom_ms * 1e-3) / 1e9
-        traffic = measured_traffic(dom_k)                # from the round's ncu capture while the kernel sources are unchanged, else null
         value = world * ncols * args.steps / dt
         e2e = world * ncols * args.steps / dt_e2e
-        line = {'metric': METRIC, 'value': value, 'unit': UNIT, 'n_gpus': world, 'steps': args.steps, 'warmup': args.warmup,
+        line = {'metric': METRIC, 'value': value, 'unit': UNIT, 'n_gpus': world, 'gpu': props.name, 'steps': args.steps, 'warmup': args.warmup,
                 'ms_per_step': 1e3 * dt / args.steps, 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': 'u8',
                 'data': 'synthetic', 'config': workload_config(args), 'clocks': clocks,
                 'e2e': {'value': e2e, 'unit': UNIT, 'h2d_bytes_per_step': h2d, 'd2h_bytes_per_step': int(out_len), 'ms_per_step': 1e3 * dt_e2e / args.steps,
                         'handles': n_h},
                 'gpu_launches': int(launches),
                 'roofline': {'bound': 'hbm', 'kernel': dom, 'achieved': achieved, 'peak': peak, 'unit': 'GB/s', 'frac': achieved / peak,
-                             'traffic': traffic, 'peak_source': peak_src, 'algorithmic_bytes_per_launch': int(alg),
+                             'traffic': None, 'peak_source': peak_src, 'algorithmic_bytes_per_launch': int(alg),
                              'bytes_in': int(bytes_in), 'bytes_out': int(out_len), 'kernel_ms': dom_ms,
                              'step_kernels_ms': {'read_stage': float(np.mean(stage_ms)), 'entry_pass': size_ms, 'tile_offset_scan': scan_ms,
                                                  'gather': write_ms, 'column_stage_total': kms, 'total': kms + float(np.mean(stage_ms))},
@@ -489,7 +496,8 @@ def main():
 
     # ------------------------------------------------------------------------------------ further BASELINE configurations
     sub = {}
-    msteps = max(3, min(args.steps, 10))
+    msteps = args.steps
+    cov_sums = None
 
     def timed(fn, k, w=2):
         for _ in range(w):
@@ -522,8 +530,8 @@ def main():
             'value': world * ncols * msteps / dtb, 'unit': UNIT, 'ms_per_step': 1e3 * dtb / msteps, 'steps': msteps, 'bytes_out': int(blen),
             'reads_per_s_baq_kernels': n_reads / (bms * 1e-3),
             'roofline': {'bound': 'fp64 (non-fused: BAQ must not contract a*b+c)', 'kernel': 'BAQ kernels (k_baq_plan + k_baq_reg)', 'achieved': ach / 1e12,
-                         'peak': FP64_NONFMA_PEAK / 1e12, 'unit': 'Top/s (FP64, non-FMA)', 'frac': ach / FP64_NONFMA_PEAK,
-                         'peak_source': 'nominal: 148 SMs x 64 FP64 lanes x 1.965 GHz (no measured FP64 figure in MEASURED_PEAKS.json)',
+                         'peak': fp64_peak and fp64_peak / 1e12, 'unit': 'Top/s (FP64, non-FMA)', 'frac': fp64_peak and ach / fp64_peak,
+                         'peak_source': f'nominal: {props.multi_processor_count} SMs x {FP64_LANES_PER_SM} FP64 lanes x max SM clock (NVML), not measured',
                          'algorithmic_ops_per_launch': ops, 'kernel_ms': bms, 'traffic': None,
                          'step_kernels_ms': {'read_stage_total': float(np.mean(st_ms[-msteps:])), 'of_which_baq': bms, 'column_stage': float(np.mean(k_ms[-msteps:]))}}}
         e.close()
@@ -554,8 +562,9 @@ def main():
             k_ms, st_ms = [], []
 
             def step_cov():
+                nonlocal cov_sums
                 e.restage(); st_ms.append(e.last_stage_device_ms)
-                e.coverage(min_baseQ=0, min_depth=1); k_ms.append(e.last_kernel_ms)
+                cov_sums = e.coverage(min_baseQ=0, min_depth=1); k_ms.append(e.last_kernel_ms)
             dtc = timed(step_cov, msteps)
             cin = int((soa['l_qseq'].astype(np.int64) + 4 * soa['n_cigar'].astype(np.int64) + 24).sum())   # qualities + cigar + core fields
             kc = float(np.mean(k_ms[-msteps:]))
@@ -601,6 +610,8 @@ def main():
                     rec, _ = cpu_leg(exe, sample, m, 1, 1, 0)
                     sub[m]['cpu_baseline'] = rec
         line['modes'] = sub
+        if args.dump_outputs:
+            dump_outputs(args.dump_outputs, last_text, cov_sums)
         print(json.dumps(line))
     eng.close(); eng_dev.close()
     if world > 1:

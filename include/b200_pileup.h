@@ -1,5 +1,5 @@
 /*
- * b200_pileup.h -- C ABI of the B200-native pileup engine (tier T2, batch API).
+ * b200_pileup.h -- C ABI of the CUDA (sm_90a) pileup engine (tier T2, batch API).
  *
  * Drop-in boundary for the mpileup / depth / coverage hot path of samtools
  * 1.23.1 (SURVEY.md section 8b).  The reference reaches this path through htslib's

@@ -1,4 +1,4 @@
-"""samtools_b200 -- B200-native mpileup / depth / coverage engine.
+"""samtools_b200 -- CUDA (sm_90a) mpileup / depth / coverage engine.
 
 The product is the CUDA library samtools_b200/lib/libb200pileup.so (C ABI in
 include/b200_pileup.h) and the CLI samtools_b200/bin/b200samtools.  This Python

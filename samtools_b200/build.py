@@ -1,10 +1,10 @@
-"""Build recipe for the native pieces (run here on CPU: nvcc cross-compiles sm_100a).
+"""Build recipe for the native pieces (nvcc cross-compiles sm_90a; no GPU is needed to build).
 
   samtools_b200/lib/libb200pileup.so   CUDA engine + C ABI (include/b200_pileup.h)
   samtools_b200/bin/b200samtools       host CLI (C++), linked against the engine
   oracle/_build/*                      CPU oracle (test infrastructure, built by its own Makefile)
 
-Everything is built in-tree so the .so/.bin travel to the GPU box with the snapshot.
+Everything is built in-tree, so the package runs from the source tree without an install step.
 """
 import os, shutil, subprocess, sys
 
@@ -13,7 +13,7 @@ CSRC = os.path.join(ROOT, 'samtools_b200', 'csrc')
 LIB = os.path.join(ROOT, 'samtools_b200', 'lib', 'libb200pileup.so')
 BIN = os.path.join(ROOT, 'samtools_b200', 'bin', 'b200samtools')
 
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-fmad=false',            # BAQ must not contract a*b+c (bit-exact with the reference's non-FMA x86 build)
               '-Xcompiler', '-fPIC', '-shared']
 
@@ -84,6 +84,7 @@ def build_read_ops_client(force=False):
 
 def build_oracle():
     subprocess.run(['make', '-s', '-C', os.path.join(ROOT, 'oracle')], check=True)
+    subprocess.run(['make', '-s', '-C', os.path.join(ROOT, 'oracle'), 'ref'], check=True)
     return os.path.join(ROOT, 'oracle', '_build', 'plp_oracle')
 
 

@@ -1,4 +1,4 @@
-// engine.cu -- B200 (sm_100a) pileup engine: device buffers, the read stage,
+// engine.cu -- H100 (sm_90a) pileup engine: device buffers, the read stage,
 // the column stage and the C ABI declared in include/b200_pileup.h.
 //
 // Data layout in HBM (one staged batch = the reads of one reference sequence
@@ -594,7 +594,7 @@ static inline int nblk(int64_t n, int t) { return (int)((n + t - 1) / t); }
 #include "overlap.cuh"
 #include "baq.cuh"
 
-extern "C" const char *b200_version(void) { return "samtools_b200 0.1 (sm_100a)"; }
+extern "C" const char *b200_version(void) { return "samtools_b200 0.1 (sm_90a)"; }
 extern "C" const char *b200_last_error(const b200_engine_t *e) { return e ? e->err : "null engine"; }
 extern "C" double b200_last_kernel_ms(const b200_engine_t *e) { return e->last_kernel_ms; }
 extern "C" double b200_last_stage_ms(const b200_engine_t *e) { return e->last_stage_ms; }

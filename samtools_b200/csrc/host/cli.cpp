@@ -94,7 +94,7 @@ struct Engine {
     bool init(int dev = -1)
     {
         if (dev < 0) { dev = 0; if (const char *s = getenv("B200_DEVICE")) dev = atoi(s); }
-        if (b200_engine_create(dev, &e) != 0) { fprintf(stderr, "b200samtools: cannot create the CUDA pileup engine (a B200/sm_100a device is required)\n"); return false; }
+        if (b200_engine_create(dev, &e) != 0) { fprintf(stderr, "b200samtools: cannot create the CUDA pileup engine (an H100/sm_90a device is required)\n"); return false; }
         return true;
     }
 };

@@ -1,4 +1,4 @@
-// hts_io.hpp -- host-side record I/O for the B200 pileup drivers (C++17, zlib only).
+// hts_io.hpp -- host-side record I/O for the pileup drivers (C++17, zlib only).
 //
 // Plays the role of the htslib calls the reference's drivers make around the
 // hot path (SURVEY.md section 2b "record I/O"): sam_open/sam_hdr_read/sam_read1,

@@ -1,5 +1,5 @@
 // plbuf_dump.cpp -- client of the reference's own bam_plbuf layer (bam_plbuf.h:32-51), which is compiled UNMODIFIED from
-// /root/reference/bam_plbuf.c against tests/compat/shim/htslib/sam.h -> include/b200_htslib_compat.h.  Shows that the
+// the reference's bam_plbuf.c against tests/compat/shim/htslib/sam.h -> include/b200_htslib_compat.h.  Shows that the
 // in-tree layer riding on the iterator API keeps working (SURVEY.md section 8b).  Same dump format as plp_dump.
 #include "fill_bam1.hpp"
 #include <cstdio>

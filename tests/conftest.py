@@ -7,7 +7,7 @@ sys.path.insert(0, ROOT)
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100, sm_90a)')
 
 
 @pytest.fixture(scope='session')

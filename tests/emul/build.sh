@@ -7,8 +7,10 @@ cd "$(dirname "$0")/../.."
 mkdir -p tests/emul/_build
 # up to date?  (every output present and no source newer than the oldest of them: four test modules call this script)
 stamp=tests/emul/_build/.stamp
+# (the objects `make -C oracle ref` compiled count as sources: plbuf_dump_emul is linked from them)
 if [ -f "$stamp" ] && [ -f tests/emul/_build/b200samtools_emul ] && [ -f tests/emul/_build/plp_dump_emul ] && [ -f tests/emul/_build/baq_host ] && \
-   [ -z "$(find samtools_b200/csrc include tests/emul tests/compat oracle -maxdepth 2 -type f \( -name '*.cpp' -o -name '*.h' -o -name '*.hpp' -o -name '*.cuh' -o -name '*.c' -o -name '*.sh' -o -name Makefile \) -newer "$stamp" 2>/dev/null | head -1)" ]; then
+   { [ ! -f oracle/_ref/ref_bam_plbuf.o ] || [ -f tests/emul/_build/plbuf_dump_emul ]; } && \
+   [ -z "$(find samtools_b200/csrc include tests/emul tests/compat oracle -maxdepth 2 -type f \( -name '*.cpp' -o -name '*.h' -o -name '*.hpp' -o -name '*.cuh' -o -name '*.c' -o -name '*.sh' -o -name Makefile -o -path 'oracle/_ref/*.o' \) -newer "$stamp" 2>/dev/null | head -1)" ]; then
     exit 0
 fi
 touch tests/emul/_build/.stamp.new.$$
@@ -17,18 +19,16 @@ g++ -std=c++17 -O1 -g -ffp-contract=off -Wall -Wno-unused-function -o tests/emul
 # the htslib-compatible iterator tier (plp_compat.cpp) + its test client, on the emulation harness
 g++ -std=c++17 -O1 -g -ffp-contract=off -Wall -Wno-unused-function -Iinclude -o tests/emul/_build/plp_dump_emul.tmp$$ \
     tests/compat/plp_dump.cpp samtools_b200/csrc/host/plp_compat.cpp samtools_b200/csrc/host/hts_io.cpp tests/emul/emul_engine.cpp -lz
-# the reference's own bam_plbuf layer, compiled UNMODIFIED where it lies (only in the dev container: /root/reference does
-# not travel) against tests/compat/shim/htslib/sam.h -> include/b200_htslib_compat.h; outputs stay under _build/
-REF=${B200_REFERENCE_DIR:-/root/reference}
-if [ -f "$REF/bam_plbuf.c" ]; then
-    gcc -c -O1 -Itests/compat/shim -Iinclude -I"$REF" -o tests/emul/_build/ref_bam_plbuf.o.tmp$$ "$REF/bam_plbuf.c"
-    g++ -std=c++17 -O1 -g -Iinclude -Itests/compat/shim -I"$REF" -o tests/emul/_build/plbuf_dump_emul.tmp$$ tests/compat/plbuf_dump.cpp \
-        tests/emul/_build/ref_bam_plbuf.o.tmp$$ samtools_b200/csrc/host/plp_compat.cpp samtools_b200/csrc/host/hts_io.cpp tests/emul/emul_engine.cpp -lz
+# the reference's own bam_plbuf layer, compiled unmodified by `make -C oracle ref` (only where a samtools source tree is
+# present), linked here against the iterator tier on the emulation harness
+if [ -f oracle/_ref/ref_bam_plbuf.o ] && [ -f oracle/_ref/plbuf_dump.o ]; then
+    g++ -std=c++17 -O1 -g -o tests/emul/_build/plbuf_dump_emul.tmp$$ oracle/_ref/plbuf_dump.o oracle/_ref/ref_bam_plbuf.o \
+        samtools_b200/csrc/host/plp_compat.cpp samtools_b200/csrc/host/hts_io.cpp tests/emul/emul_engine.cpp -lz
 fi
 # the register-band BAQ arithmetic (samtools_b200/csrc/baq_reg.h) single-stepped on the CPU against the oracle's sam_prob_realn
 make -s -C oracle
 g++ -std=c++17 -O2 -ffp-contract=off -Wno-unknown-pragmas -o tests/emul/_build/baq_host.tmp$$ tests/emul/baq_host.cpp \
     -Loracle/_build -loracle -Wl,-rpath,"$PWD/oracle/_build" -lz -lm
 
-for f in b200samtools_emul baq_host plbuf_dump_emul plp_dump_emul ref_bam_plbuf.o; do if [ -f tests/emul/_build/$f.tmp$$ ]; then mv -f tests/emul/_build/$f.tmp$$ tests/emul/_build/$f; fi; done
+for f in b200samtools_emul baq_host plbuf_dump_emul plp_dump_emul; do if [ -f tests/emul/_build/$f.tmp$$ ]; then mv -f tests/emul/_build/$f.tmp$$ tests/emul/_build/$f; fi; done
 mv -f tests/emul/_build/.stamp.new.$$ tests/emul/_build/.stamp

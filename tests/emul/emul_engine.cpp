@@ -4,7 +4,7 @@
 // __host__ __device__ per-read / per-column functions the CUDA kernels call
 // (samtools_b200/csrc/plp_core.h, plp_stage.h) in a plain single-threaded
 // loop.  It exists so that the column arithmetic and the host drivers can be
-// debugged in the dev container, which has no GPU.  It is built only by
+// debugged on a machine without a GPU.  It is built only by
 // tests/emul/build.sh, is never linked into libb200pileup.so or b200samtools,
 // is never used as a fallback, and is not a measured or shipped path.
 // BAQ (warp-cooperative kernel) and GL are NOT emulated: calls needing them fail.

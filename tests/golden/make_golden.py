@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """Bundle the reference's own pileup test corpus into tests/golden/ref_corpus.tar.gz.
 
-/root/reference does not exist on the GPU box, so the golden inputs (small
+The reference tree does not travel with this repository, so the golden inputs (small
 SAM/BAM/FASTA/BED fixtures) and the expected outputs that pin the hot path
 (SURVEY.md section 8c) are packed here, once, by this script:
 
@@ -13,11 +13,13 @@ SAM/BAM/FASTA/BED fixtures) and the expected outputs that pin the hot path
   test/bedcov/*, examples/{ex1.fa,ex1.sam.gz,toy.*}
 
 Nothing here is reference SOURCE code; these are data files of the
-reference's test-suite.  Run:  python tests/golden/make_golden.py
+reference's test-suite.  Run:  python tests/golden/make_golden.py <samtools source tree>
 """
 import os, tarfile, io, sys, glob
 
-REF = sys.argv[1] if len(sys.argv) > 1 else '/root/reference'
+if len(sys.argv) != 2:
+    sys.exit('usage: make_golden.py <samtools source tree>')
+REF = sys.argv[1]
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'ref_corpus.tar.gz')
 
 def want(path):

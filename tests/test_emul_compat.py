@@ -38,11 +38,11 @@ def test_iterator_hooks_and_kstring_insertion(args, files, dump_emul, oracle_bin
 @pytest.mark.parametrize('f', ['test/mpileup/mp_DI.sam', 'test/mpileup/mp_N2.sam', 'test/mpileup/mpileup.1.bam'])
 def test_reference_bam_plbuf_rides_on_the_tier(f, dump_emul, oracle_bin, corpus):
     """The reference's own bam_plbuf.c (bam_plbuf.h:32-51), compiled unmodified against the compatibility header, drives
-    the iterator tier through bam_plp_push / bam_plp64_next and sees the columns htslib would hand it.  Needs the
-    reference tree, so it runs in the dev container only."""
+    the iterator tier through bam_plp_push / bam_plp64_next and sees the columns htslib would hand it.  Needs the objects
+    `make -C oracle ref` compiles from a samtools source tree."""
     exe = os.path.join(ROOT, 'tests', 'emul', '_build', 'plbuf_dump_emul')
-    if not os.path.exists(exe) or not os.path.exists(os.environ.get('B200_REFERENCE_DIR', '/root/reference') + '/bam_plbuf.c'):
-        pytest.skip('reference tree not present (GPU box): bam_plbuf.c cannot be compiled here')
+    if not os.path.exists(os.path.join(ROOT, 'oracle', '_ref', 'ref_bam_plbuf.o')):
+        pytest.skip('oracle/_ref/ref_bam_plbuf.o absent: no samtools source tree to compile bam_plbuf.c from')
     got = subprocess.run([exe, os.path.join(corpus, f)], capture_output=True)
     want = subprocess.run([oracle_bin, 'pileup-dump', os.path.join(corpus, f)], capture_output=True)
     assert got.returncode == 0, got.stderr[-300:]

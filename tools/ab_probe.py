@@ -1,4 +1,4 @@
-"""A/B timing of engine variants in ONE process launch per variant (development aid; keeps gpurun calls short).
+"""A/B timing of engine variants in ONE process launch per variant (development aid; keeps GPU runs short).
 
   python tools/ab_probe.py [--mb 8] [--reps 5] label[:ENV=V[,ENV=V...]] ...
   e.g.  python tools/ab_probe.py default general:B200_PLP_GENERAL=1 vec:B200_PLP_TMA=0

@@ -1,6 +1,6 @@
-// fp64_probe.cu -- development aid: non-fused FP64 issue rate and dependent-issue latency of one B200, the
+// fp64_probe.cu -- development aid: non-fused FP64 issue rate and dependent-issue latency of one GPU, the
 // denominator of the BAQ roofline (SURVEY.md 8d: BAQ must not contract a*b+c, so an FMA slot carries ONE operation).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -fmad=false -o tools/_build/fp64_probe tools/fp64_probe.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -fmad=false -o tools/_build/fp64_probe tools/fp64_probe.cu
 #include <cuda_runtime.h>
 #include <stdio.h>
 #include <stdlib.h>

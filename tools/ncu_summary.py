@@ -1,5 +1,5 @@
 """Condense an .ncu-rep (ncu --set full) into the text summary kept under profiles/.
-  python tools/ncu_summary.py gpurun_out/prof.ncu-rep profiles/r01_xxx.txt ["note"]"""
+  python tools/ncu_summary.py prof.ncu-rep profiles/<name>.txt ["note"]"""
 import csv, io, subprocess, sys
 
 KEYS = ['gpu__time_duration.sum', 'launch__grid_size', 'launch__block_size', 'launch__registers_per_thread',
