@@ -438,6 +438,20 @@ static int read_bam_rec(reader_t *rd, rec_t *r)
     r->l_aux = (int)(d + bs - p);
     r->aux = dupmem(p, (size_t)r->l_aux);
     free(d);
+    /* SAMv1 4.2.2: a CIGAR of more than 65535 ops is stored in a CG:B,I tag; the record's own CIGAR is then the
+       placeholder <l_qseq>S <rlen>N.  The tag's ops become the CIGAR and the tag is dropped. */
+    if (r->n_cigar == 2 && (r->cigar[0] & 0xf) == 4 && (int32_t)(r->cigar[0] >> 4) == r->l_qseq && (r->cigar[1] & 0xf) == 3) {
+        const uint8_t *cg = rec_aux_get(r, "CG");
+        if (cg && cg[0] == 'B' && cg[1] == 'I') {
+            uint32_t nc; memcpy(&nc, cg + 2, 4);
+            if (nc > 0 && cg + 6 + 4 * (size_t)nc <= r->aux + r->l_aux) {
+                uint32_t *ops = malloc(4 * (size_t)nc);
+                memcpy(ops, cg + 6, 4 * (size_t)nc);
+                free(r->cigar); r->cigar = ops; r->n_cigar = nc;
+                rec_aux_del(r, cg);
+            }
+        }
+    }
     return 0;
 }
 

@@ -471,10 +471,9 @@ int launch_baq(b200_engine *e, const RawSoA &r, const b200_stage_conf_t &cf)
     int32_t *idx = e->baq_idx, *idx2 = e->baq_idx + nr;
     BaqPlan *plan = (BaqPlan *)(e->baq_idx + 2 * nr);
     // band-7 reads run on the register kernel (k_baq_reg), everything else (wide bands, very long reads) on the warp kernel;
-    // B200_BAQ_REG=0 sends every read to the warp kernel (cross-check)
-    static const int use_reg = getenv("B200_BAQ_REG") ? atoi(getenv("B200_BAQ_REG")) : 1;
+    // B200_BAQ_REG=0 (read per handle when it is created) sends every read to the warp kernel (cross-check)
     CK(cudaMemsetAsync(e->d_misc + 16, 0, 16 * 8, e->stream));
-    k_baq_plan<<<nblk(n, 256), 256, 0, e->stream>>>(r, cf, e->state, plan, idx, idx2, use_reg, e->d_misc + 16); e->launches++;
+    k_baq_plan<<<nblk(n, 256), 256, 0, e->stream>>>(r, cf, e->state, plan, idx, idx2, e->baq_reg, e->d_misc + 16); e->launches++;
     unsigned long long h[5];
     CK(cudaMemcpyAsync(h, e->d_misc + 16, sizeof h, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));

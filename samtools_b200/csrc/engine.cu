@@ -627,6 +627,7 @@ extern "C" int b200_engine_create(int device, b200_engine_t **out)
     const char *s = getenv("B200_PLP_SMEM_TEXT"); if (s) e->smem_text = (uint32_t)atoi(s);
     s = getenv("B200_PLP_TMA"); e->use_tma = s ? atoi(s) : 1;
     s = getenv("B200_PLP_GENERAL"); e->general = s ? atoi(s) : 0;   // 1: general mpileup path (thread-per-column size + write) for every configuration
+    s = getenv("B200_BAQ_REG"); e->baq_reg = s ? atoi(s) : 1;
     if (e->smem_text + 16 > 48 * 1024) {   // the attribute is per function and process-wide: only ever raise it (another handle may use more)
         cudaFuncSetAttribute(k_mp_gather<7, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
         cudaFuncSetAttribute(k_mp_gather<7, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);

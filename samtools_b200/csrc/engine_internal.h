@@ -24,6 +24,7 @@ struct b200_engine {
     void *d_gfmt = nullptr;      // device copy of the gather's parameter block (cold paths)
     bool baq_attr_set = false;   // k_baq_reg's dynamic shared-memory attribute has been raised on this handle's device
     int use_tma = 1, general = 0;
+    int baq_reg = 1;             // 0: every BAQ read on the warp kernel k_baq (B200_BAQ_REG, cross-check of k_baq_reg)
 
     // raw SoA image of the staged records
     DBUF(int64_t, pos); DBUF(uint16_t, flag); DBUF(uint8_t, mapq); DBUF(int32_t, l_qseq); DBUF(uint32_t, n_cigar);

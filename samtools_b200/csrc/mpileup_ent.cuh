@@ -175,11 +175,14 @@ constexpr int ENT_PAD = 64;
 
 // cold paths read the View / configuration from a copy in global memory: taking the address of the kernel parameter for an
 // out-of-line call would make every thread copy the whole parameter block to local memory
-__device__ __noinline__ int ent_special_g(const MpEntFmt *g, int32_t i, int32_t c, char *ps)
+// Length and quality come back as separate fields: the text of a deletion entry includes the deleted reference bases, so a
+// long deletion's entry is longer than 16 bits.
+struct SpecialEnt { uint32_t n; int q; };
+__device__ __noinline__ SpecialEnt ent_special_g(const MpEntFmt *g, int32_t i, int32_t c, char *ps)
 {
-    int q;
-    const int n = ent_special(g->v, g->cf, i, c, ps, q);
-    return n | q << 16;
+    SpecialEnt r;
+    r.n = (uint32_t)ent_special(g->v, g->cf, i, c, ps, r.q);
+    return r;
 }
 
 constexpr int GROW = 88;                       // bytes per row: 80 fetched + 8 so that 8-byte stores of consecutive lanes hit distinct banks
@@ -257,9 +260,9 @@ __device__ __forceinline__ void gather_group(const MpEntFmt &fmt, const MpEntFmt
                     const uint32_t mapq = (hw.z >> 16) & 0xffu;
                     if (e & 0x8080u) {                                   // "^" / "$" decorations or indel text: rare
                         if (e == ENT_SPECIAL) {
-                            const int rq = ent_special_g(gfmt, (int32_t)hw.w, c, sb + (so - sb_s));
-                            so += (uint32_t)(rq & 0xffff);
-                            const int q = rq >> 16;
+                            const SpecialEnt se = ent_special_g(gfmt, (int32_t)hw.w, c, sb + (so - sb_s));
+                            so += se.n;
+                            const int q = se.q;
                             sts8(qo++, (uint32_t)(q + 33 < 126 ? q + 33 : 126));
                         } else {
                             if (e & 0x80u) { sts8(so++, (uint32_t)'^'); sts8(so++, umin32(mapq + 33u, 126u)); }

@@ -207,7 +207,11 @@ def write_fasta(path, name, ref, width=60):
 
 
 def write_sam(path, soa, max_reads=None):
-    """The same records as SAM text (names p%09d, so the name-hash bit matches rbits)."""
+    """The same records as SAM text (names p%09d, so the name-hash bit matches rbits).
+    A list of batches (one per contig, as make_long_set returns) or a batch of variable-length reads goes through
+    _write_sam_var."""
+    if isinstance(soa, (list, tuple)) or soa.get('read_len') is None:
+        return _write_sam_var(path, soa if isinstance(soa, (list, tuple)) else [soa])
     name = soa['tid_name']; L = soa['read_len']
     lq = L + (L & 1)
     n = len(soa['pos']) if max_reads is None else min(max_reads, len(soa['pos']))
@@ -251,6 +255,8 @@ def take_reads(soa, idx):
     leave the selection become -1.  All reads must have the same l_qseq (true of this generator)."""
     idx = np.asarray(idx, dtype=np.int64)
     n0 = len(soa['pos'])
+    if soa.get('read_len') is None:
+        return _take_reads_var(soa, idx)
     L = soa['read_len']; lq = L + (L & 1)
     out = dict(soa)
     for k in ('pos', 'flag', 'mapq', 'l_qseq', 'n_cigar', 'mtid', 'mpos', 'isize', 'rbits', 'pair_id'):
@@ -326,7 +332,10 @@ def _reg2bin(beg, end):
 
 def write_bam(path, soa, level=1, block=0xff00):
     """The same records as a coordinate-sorted BAM (BGZF, SAMv1 4.2): what `samtools mpileup` really reads.
-    Names are p%09d like write_sam().  No index is written (the readers here scan)."""
+    Names are p%09d like write_sam().  No index is written (the readers here scan).
+    A list of batches or a batch of variable-length reads goes through _write_bam_var."""
+    if isinstance(soa, (list, tuple)) or soa.get('read_len') is None:
+        return _write_bam_var(path, soa if isinstance(soa, (list, tuple)) else [soa], level, block)
     import struct
     import zlib
     name = soa['tid_name'].encode(); L = soa['read_len']; lq = L + (L & 1)
@@ -367,7 +376,12 @@ def write_bam(path, soa, level=1, block=0xff00):
     buf[(so[:, None] + np.arange(seq.shape[1])[None, :]).reshape(-1)] = seq.reshape(-1)
     qo = so + seq.shape[1]
     buf[(qo[:, None] + np.arange(L)[None, :]).reshape(-1)] = qual.reshape(-1)
-    data = hdr + buf.tobytes()
+    _write_bgzf(path, hdr + buf.tobytes(), level, block)
+
+
+def _write_bgzf(path, data, level, block):
+    import struct
+    import zlib
     with open(path, 'wb') as f:
         for i in range(0, len(data), block):
             chunk = data[i:i + block]
@@ -376,3 +390,372 @@ def write_bam(path, soa, level=1, block=0xff00):
             f.write(b'\x1f\x8b\x08\x04\0\0\0\0\0\xff\x06\0BC\x02\0' + struct.pack('<H', len(comp) + 25) + comp +
                     struct.pack('<II', zlib.crc32(chunk) & 0xffffffff, len(chunk)))
         f.write(bytes.fromhex('1f8b08040000000000ff0600424302001b0003000000000000000000'))
+
+
+# ---------------------------------------------------------------------------------------------------------- long reads
+# Variable-length batches: 'read_len' is None, every read has its own l_qseq; qualities start on even offsets (qual_off) and
+# the bases are the nibbles qual_off.. of seq4, as b200_batch_t requires.
+_OPS = 'MIDNSHP=XB'
+_QCONS = np.array([1, 1, 0, 0, 1, 0, 0, 1, 1, 0], dtype=bool)      # M I D N S H P = X B: consumes query
+_RCONS = np.array([1, 0, 1, 1, 0, 0, 0, 1, 1, 0], dtype=bool)      # consumes reference
+
+
+def parse_cigar(s):
+    """'300M2I10D' -> (lengths, op codes) as int64 arrays"""
+    import re
+    t = re.findall(r'(\d+)([MIDNSHP=XB])', s)
+    return np.array([int(l) for l, _ in t], dtype=np.int64), np.array([_OPS.index(o) for _, o in t], dtype=np.int64)
+
+
+def baq_band(pos, lens, ops, lq, ref_len):
+    """Band probaln_glocal runs with for one read under sam_prob_realn's window rule (None: the read gets no HMM -- an N
+    skip, or no M op).  Restated here for the generator's self-checks: it classifies inputs, it does not compute answers."""
+    x = int(pos); xb = xe = -1; y = 0; yb = ye = -1
+    for l, op in zip(lens.tolist(), ops.tolist()):
+        if op in (0, 7, 8):
+            if yb < 0: yb = y
+            if xb < 0: xb = x
+            ye = y + l; xe = x + l; x += l; y += l
+        elif op in (1, 4): y += l
+        elif op == 2: x += l
+        elif op == 3: return None
+    if xb == -1:
+        return None
+    bw = 7
+    dd = abs((xe - xb) - (ye - yb))
+    if dd > bw: bw = dd + 3
+    xb = max(xb - (yb + bw // 2), 0)
+    xe += lq - ye + bw // 2
+    if xe - xb - lq > bw:
+        xb += (xe - xb - lq - bw) // 2
+        xe -= (xe - xb - lq - bw) // 2
+    xe = min(xe, ref_len)
+    l_ref = xe - xb
+    if l_ref <= 0:
+        return None
+    return max(min(max(l_ref, lq), bw), abs(l_ref - lq))
+
+
+def _realise(rng, ref, pos, lens, ops, sub_rate=0.03, n_rate=0.002):
+    """query bases of a read with this CIGAR at `pos`: the reference under aligned ops (plus substitutions), random bases in
+    insertions / soft clips / past the contig end, some N"""
+    ql = np.where(_QCONS[ops], lens, 0); rl = np.where(_RCONS[ops], lens, 0)
+    rstart = pos + np.concatenate([[0], np.cumsum(rl)[:-1]])
+    qstart = np.concatenate([[0], np.cumsum(ql)[:-1]])
+    n = int(ql.sum())
+    ridx = np.repeat(rstart - qstart, ql) + np.arange(n)
+    ok = np.repeat(np.isin(ops, (0, 7, 8)), ql) & (ridx >= 0) & (ridx < len(ref))
+    acgt = np.frombuffer(b'ACGT', dtype=np.uint8)
+    base = acgt[rng.integers(0, 4, n)]
+    base[ok] = ref[ridx[ok]]
+    sub = ok & (rng.random(n) < sub_rate)
+    base[sub] = acgt[rng.integers(0, 4, int(sub.sum()))]
+    base[rng.random(n) < n_rate] = ord('N')
+    return base
+
+
+def _long_quals(rng, n, mode='ont'):
+    if mode == 'star':
+        return np.full(n, 0xff, dtype=np.uint8)
+    if mode == 'wide':
+        return (np.arange(n) % 94).astype(np.uint8)
+    q = np.clip(np.rint(rng.normal(18.0, 8.0, n)), 0, 93).astype(np.uint8)
+    u = rng.random(n)
+    q[u < 0.02] = 93; q[u > 0.99] = 0
+    return q
+
+
+def _ont_cigar(rng, span, indel_rate=0.03, del_bias=0.0, max_run=6):
+    """M runs separated by single I / D events (geometric lengths <= max_run) covering ~span reference bases.
+    del_bias in (-1, 1) tilts the events towards deletions (> 0) or insertions (< 0): the net indel difference, and with it
+    the BAQ band, grows with |del_bias|."""
+    n_ev = int(span * indel_rate * 1.5) + 8
+    m = rng.geometric(indel_rate, n_ev).astype(np.int64)
+    is_del = rng.random(n_ev) < 0.5 * (1.0 + del_bias)
+    il = np.minimum(rng.geometric(0.55, n_ev), max_run).astype(np.int64)
+    k = min(int(np.searchsorted(np.cumsum(m + np.where(is_del, il, 0)), span)) + 1, n_ev)
+    lens = np.empty(2 * k - 1, dtype=np.int64); ops = np.zeros(2 * k - 1, dtype=np.int64)
+    lens[0::2] = m[:k]
+    lens[1::2] = il[:k - 1]; ops[1::2] = np.where(is_del[:k - 1], 2, 1)
+    return lens, ops
+
+
+def _rec(rng, ref, pos, lens, ops, flag=0, name=None, qmode='ont', mapq=60, **kw):
+    seq = _realise(rng, ref, pos, lens, ops, **kw)
+    return dict(pos=int(pos), lens=lens, ops=ops, flag=int(flag), name=name, mapq=int(mapq), seq=seq, qual=_long_quals(rng, len(seq), qmode))
+
+
+def _pack(recs, ref, length, tid, tid_name, name_base=0):
+    """records -> variable-length SoA (coordinate sorted, stable); names p%09d of name_base + record['name'] (reads without a
+    name get a fresh one); mates are the records sharing a name (their mate fields point at the next one, cyclically)"""
+    nxt = max([r['name'] for r in recs if r['name'] is not None] + [-1]) + 1
+    for r in recs:
+        if r['name'] is None:
+            r['name'] = nxt; nxt += 1
+    recs = sorted(recs, key=lambda r: r['pos'])
+    n = len(recs)
+    pos = np.array([r['pos'] for r in recs], dtype=np.int64)
+    lq = np.array([len(r['seq']) for r in recs], dtype=np.int32)
+    ncig = np.array([len(r['lens']) for r in recs], dtype=np.uint32)
+    cigar = np.concatenate([(r['lens'] << 4) | r['ops'] for r in recs]).astype(np.uint32)
+    cigar_off = np.concatenate([[0], np.cumsum(ncig.astype(np.int64))[:-1]]).astype(np.uint64)
+    padded = lq.astype(np.int64) + (lq & 1)
+    qo = np.concatenate([[0], np.cumsum(padded)[:-1]]).astype(np.int64)
+    tot = int(padded.sum())
+    qual = np.zeros(tot + 2, dtype=np.uint8); nib = np.zeros(tot + 2, dtype=np.uint8)
+    lut = np.full(256, 15, dtype=np.uint8)
+    for ch, v in NT16.items():
+        lut[ord(ch)] = v
+    for i, r in enumerate(recs):
+        qual[qo[i]:qo[i] + lq[i]] = r['qual']; nib[qo[i]:qo[i] + lq[i]] = lut[r['seq']]
+    seq4 = (nib[0::2] << 4) | nib[1::2]
+    pair_id = np.array([name_base + r['name'] for r in recs], dtype=np.int64)
+    flag = np.array([r['flag'] for r in recs], dtype=np.uint16)
+    rlen = np.array([int(r['lens'][_RCONS[r['ops']]].sum()) for r in recs], dtype=np.int64)
+    prev = np.full(n, -1, dtype=np.int64); mtid = np.full(n, -1, dtype=np.int32)
+    mpos = np.full(n, -1, dtype=np.int64); isize = np.zeros(n, dtype=np.int64)
+    groups = {}
+    for i in range(n):
+        g = groups.setdefault(int(pair_id[i]), [])
+        if g:
+            prev[i] = g[-1]
+        g.append(i)
+    for g in groups.values():
+        if len(g) < 2:
+            continue
+        lo = min(pos[g]); hi = max(pos[g] + rlen[g])
+        for k, i in enumerate(g):
+            if flag[i] & 1:
+                j = g[(k + 1) % len(g)]
+                mtid[i] = tid; mpos[i] = pos[j]
+                isize[i] = (hi - lo) if pos[i] == lo and k == 0 else -(hi - lo)
+    return dict(file_start=np.array([0, n], dtype=np.int64), pos=pos, flag=flag, mapq=np.array([r['mapq'] for r in recs], dtype=np.uint8),
+                l_qseq=lq, n_cigar=ncig, cigar_off=cigar_off, qual_off=qo.astype(np.uint64), mtid=mtid, mpos=mpos, isize=isize,
+                prev_same_name=prev, rbits=(_name_odd(pair_id) * 2).astype(np.uint8), cigar=cigar, seq4=np.ascontiguousarray(seq4),
+                qual=qual, tid=tid, tid_len=length, tid_name=tid_name, ref=ref, ref_beg=0, ref_len=length, pair_id=pair_id,
+                read_len=None, ref_full=ref)
+
+
+def _band_cigar(pos, ref_len, target):
+    """300M<k>D300M or 300M<k>I300M whose BAQ band is exactly `target`"""
+    for k in range(1, 1000):
+        for op in 'DI':
+            s = f'300M{k}{op}300M'
+            lens, ops = parse_cigar(s)
+            if baq_band(pos, lens, ops, 600 + (k if op == 'I' else 0), ref_len) == target:
+                return s
+    raise ValueError(target)
+
+
+def _name_with_parity(start, parity):
+    i = start
+    while int(_name_odd(np.array([i]))[0]) != parity:
+        i += 1
+    return i
+
+
+def _planted(rng, ref, length):
+    """the long-read edge cases (positions inside a contig of >= 160 kb)"""
+    P = []
+    add = lambda pos, cig, **kw: P.append(_rec(rng, ref, pos, *parse_cigar(cig), **kw))
+    # l_qseq 1 / 8 / 9 / 511 / 512 / 513 (band 7: 512 on the register kernel, 513 on the warp kernel)
+    for k, l in enumerate((1, 8, 9, 511, 512, 513)):
+        add(5000 + 700 * k, f'{l}M')
+    # n_cigar 8 and 9 (hard + soft clips)
+    add(10_000, '10S100M2I100M3D100M1I90M', flag=16)
+    add(10_050, '5H10S100M2I100M3D100M1I90M')
+    # reference spans 511 / 512 / 513 / 544, simple and with an insertion / a deletion
+    for k, s in enumerate((511, 512, 513, 544)):
+        add(11_000 + 97 * k, f'{s}M')
+        add(11_010 + 97 * k, f'200M3I{s - 200}M', flag=16)
+        add(11_020 + 97 * k, f'200M4D{s - 204}M')
+    # BAQ bands of 15 / 16 / 31 / 32 / 100 (2*bw+1 = 31 / 33 / 63 / 65 / 201 cells: both sides of the 32- and 64-cell edges)
+    for k, b in enumerate((15, 16, 31, 32, 100)):
+        add(13_000 + 1500 * k, _band_cigar(13_000 + 1500 * k, length, b))
+    # leading soft clips of 65535 / 65536 on <n>M reads (the clip decides the simple-read qstart)
+    add(100_000, '65535S400M')
+    add(100_500, '65536S400M', flag=16)
+    # hard clips
+    add(21_000, '30H500M'); add(21_100, '500M40H', flag=16); add(21_200, '10H20S400M15S10H')
+    # deletions of >= 512 bases (the 1000-base one covers whole 32-column groups as '*' only)
+    add(22_000, '300M1000D300M'); add(22_100, '200M600D200M', flag=16)
+    # N skips of several kb (no BAQ)
+    add(24_000, '500M3000N500M'); add(24_200, '400M5000N300M', flag=16)
+    # an insertion of 2 kb
+    add(30_500, '300M2100I300M')
+    # qualities 0..93, '*' qualities, N bases
+    add(31_000, '700M', qmode='wide'); add(31_100, '800M', qmode='star'); add(31_200, '600M', n_rate=0.1)
+    # position 0, and a read running past the contig end
+    add(0, '300M'); add(0, '20S300M', flag=16); add(length - 150, '400M')
+    # overlapping long mates: both simple, one with indels, both with indels; both name-hash parities; one name triplet
+    nm = 900_000
+    for k, (a, b, par) in enumerate((('3000M', '3000M', 0), ('3000M', '3000M', 1), ('1000M5D1000M3I997M', '2500M', 0),
+                                     ('2500M', '1200M8I1300M', 1), (None, None, 0), (None, None, 1))):
+        nm = _name_with_parity(nm + 1, par)
+        p0 = 40_000 + 8000 * k
+        la, oa = parse_cigar(a) if a else _ont_cigar(rng, 4000)
+        lb, ob = parse_cigar(b) if b else _ont_cigar(rng, 4000)
+        f0, f1 = (99, 147) if k % 2 == 0 else (163, 83)
+        P.append(_rec(rng, ref, p0, la, oa, flag=f0, name=nm))
+        P.append(_rec(rng, ref, p0 + 1500, lb, ob, flag=f1, name=nm))
+    nm = _name_with_parity(nm + 1, 0)
+    for k, (cig, f) in enumerate((('2000M', 99), ('1500M10D500M', 147), ('2000M', 2048 | 97))):
+        add(90_000 + 600 * k, cig, flag=f, name=nm)
+    return P
+
+
+def make_long_reads(length=200_000, depth=12, seed=31, ref=None, ref_seed=None, tid=0, tid_name='chr1', del_bias=0.0,
+                    indel_rate=0.03, sub_rate=0.03, median_len=2500, sigma=0.8, max_len=40_000, frac_pair=0.12,
+                    plant=True, name_base=0):
+    """ONT/PacBio-like reads on one contig, as a variable-length SoA (read_len None; see make_batch for the fields).
+      lengths    log-normal around median_len, clipped to 513 .. max_len
+      errors     substitutions (sub_rate) and single I / D runs of <= 6 bases (indel_rate per base, del_bias tilts them)
+      clips      20 % soft clip on each side (10..500 bases), 5 % hard clips
+      qualities  ~N(18, 8) clipped to 0..93 with spikes at 0 and 93; 2 % of reads '*'; 0.2 % N bases
+      mates      frac_pair of the reads get an overlapping long mate (99/147 or 163/83)
+      plant      adds every edge case of _planted (needs length >= 160 kb)
+    Seeded: the same arguments give the same batch."""
+    rng = np.random.default_rng(seed)
+    if ref is None:
+        ref = make_reference(length, seed * 7 + 3 if ref_seed is None else ref_seed)
+    recs = _planted(rng, ref, length) if plant else []
+    n_reads = int(round(depth * length / float(median_len) / np.exp(sigma * sigma / 2)))
+    for _ in range(n_reads):
+        span = int(np.clip(rng.lognormal(np.log(median_len), sigma), 513, max_len))
+        span = min(span, length - 10)
+        pos = int(rng.integers(0, max(1, length - span)))
+        lens, ops = _ont_cigar(rng, span, indel_rate, del_bias)
+        if rng.random() < 0.2: lens, ops = np.concatenate([[rng.integers(10, 500)], lens]), np.concatenate([[4], ops])
+        if rng.random() < 0.2: lens, ops = np.concatenate([lens, [rng.integers(10, 500)]]), np.concatenate([ops, [4]])
+        if rng.random() < 0.05: lens, ops = np.concatenate([[rng.integers(1, 2000)], lens]), np.concatenate([[5], ops])
+        u = rng.random()
+        flag = 1024 if u < 0.005 else 256 if u < 0.01 else 0
+        qmode = 'star' if rng.random() < 0.02 else 'ont'
+        mapq = 60 if rng.random() < 0.9 else int(rng.integers(0, 60))
+        if rng.random() < frac_pair:
+            nm = len(recs) + 1_000_000
+            mp = pos + int(span * rng.uniform(0.1, 0.9))
+            mspan = min(int(np.clip(rng.lognormal(np.log(median_len), sigma), 513, max_len)), length - 10 - mp)
+            f0, f1 = (99, 147) if rng.random() < 0.5 else (163, 83)
+            recs.append(_rec(rng, ref, pos, lens, ops, flag=f0, name=nm, qmode=qmode, mapq=mapq, sub_rate=sub_rate))
+            if mspan > 50:
+                ml, mo = _ont_cigar(rng, mspan, indel_rate, del_bias)
+                recs.append(_rec(rng, ref, mp, ml, mo, flag=f1, name=nm, mapq=mapq, sub_rate=sub_rate))
+            continue
+        recs.append(_rec(rng, ref, pos, lens, ops, flag=flag | (16 if rng.random() < 0.5 else 0), qmode=qmode, mapq=mapq, sub_rate=sub_rate))
+    return _pack(recs, ref, length, tid, tid_name, name_base)
+
+
+def make_long_set(seed=31, lengths=(200_000, 120_000), **kw):
+    """two contigs of long reads (chr1 carries the planted edge cases); write_sam / write_bam take the list"""
+    out = []
+    plant = kw.pop('plant', True)
+    for t, L in enumerate(lengths):
+        out.append(make_long_reads(length=L, seed=seed + 1000 * t, tid=t, tid_name=f'chr{t + 1}', plant=plant and t == 0,
+                                   name_base=10_000_000 * t, **kw))
+    return out
+
+
+def make_long_deletion(seed=41, length=100_000, del_len=70_000):
+    """a small input whose one read carries a `del_len`-base deletion (its mpileup entry is longer than 64 KiB), at low depth
+    around it.  Only for -B: with BAQ on, that read's band would need gigabytes."""
+    rng = np.random.default_rng(seed)
+    ref = make_reference(length, seed * 7 + 3)
+    recs = [_rec(rng, ref, 10_000, *parse_cigar(f'300M{del_len}D300M'))]
+    recs[0]['qual'][:] = 30                   # its entry before the deletion passes the default -Q 13
+    for k in range(40):
+        p = int(rng.integers(0, length - 700))
+        recs.append(_rec(rng, ref, p, *parse_cigar('600M'), flag=16 if k & 1 else 0))
+    return _pack(recs, ref, length, 0, 'chr1')
+
+
+def make_long_cigar(seed=43, length=120_000, n_rep=16_500):
+    """a small input with one read of 4 * n_rep > 65535 CIGAR ops (write_bam stores it as CG:B,I behind the
+    <l_qseq>S<rlen>N placeholder), plus a few long reads around it"""
+    rng = np.random.default_rng(seed)
+    ref = make_reference(length, seed * 7 + 3)
+    lens = np.tile(np.array([2, 1, 2, 1], dtype=np.int64), n_rep); ops = np.tile(np.array([0, 1, 0, 2], dtype=np.int64), n_rep)
+    recs = [_rec(rng, ref, 1000, lens, ops)]
+    for k in range(30):
+        span = int(rng.integers(600, 6000))
+        l, o = _ont_cigar(rng, span)
+        recs.append(_rec(rng, ref, int(rng.integers(0, length - span)), l, o, flag=16 if k & 1 else 0))
+    return _pack(recs, ref, length, 0, 'chr1')
+
+
+def _nibbles(soa):
+    s = soa['seq4']
+    nib = np.empty(2 * len(s), dtype=np.uint8); nib[0::2] = s >> 4; nib[1::2] = s & 15
+    return nib
+
+
+def _write_sam_var(path, soas):
+    with open(path, 'w') as f:
+        f.write('@HD\tVN:1.6\tSO:coordinate\n' + ''.join(f'@SQ\tSN:{s["tid_name"]}\tLN:{s["tid_len"]}\n' for s in soas))
+        for soa in soas:
+            name = soa['tid_name']; nib = _nibbles(soa)
+            for i in range(len(soa['pos'])):
+                co = int(soa['cigar_off'][i]); nc = int(soa['n_cigar'][i])
+                c = soa['cigar'][co:co + nc]
+                cg = ''.join(f'{l}{_OPS[o]}' for l, o in zip((c >> 4).tolist(), (c & 15).tolist()))
+                qo = int(soa['qual_off'][i]); l = int(soa['l_qseq'][i])
+                seq = _CODE2CH[nib[qo:qo + l]].tobytes().decode() if l else '*'
+                q = soa['qual'][qo:qo + l]
+                ql = '*' if l == 0 or q[0] == 0xff else (q + 33).tobytes().decode()
+                mt = int(soa['mtid'][i])
+                f.write(f'p{int(soa["pair_id"][i]):09d}\t{int(soa["flag"][i])}\t{name}\t{int(soa["pos"][i]) + 1}\t{int(soa["mapq"][i])}\t{cg}\t'
+                        f'{"*" if mt < 0 else "="}\t{int(soa["mpos"][i]) + 1}\t{int(soa["isize"][i])}\t{seq}\t{ql}\n')
+
+
+def _write_bam_var(path, soas, level, block):
+    """write_bam for variable-length reads; a CIGAR of more than 65535 ops goes into CG:B,I behind <l_qseq>S<rlen>N (SAMv1 4.2.2)"""
+    import struct
+    text = ('@HD\tVN:1.6\tSO:coordinate\n' + ''.join(f'@SQ\tSN:{s["tid_name"]}\tLN:{s["tid_len"]}\n' for s in soas)).encode()
+    out = [b'BAM\1' + struct.pack('<i', len(text)) + text + struct.pack('<i', len(soas))]
+    for s in soas:
+        nm = s['tid_name'].encode()
+        out.append(struct.pack('<i', len(nm) + 1) + nm + b'\0' + struct.pack('<i', int(s['tid_len'])))
+    for s in soas:
+        nib = _nibbles(s); rl = ref_span(s)
+        for i in range(len(s['pos'])):
+            co = int(s['cigar_off'][i]); nc = int(s['n_cigar'][i]); l = int(s['l_qseq'][i]); qo = int(s['qual_off'][i])
+            cig = s['cigar'][co:co + nc].astype('<u4')
+            aux = b''
+            if nc > 65535:
+                aux = b'CGBI' + struct.pack('<I', nc) + cig.tobytes()
+                cig = np.array([(l << 4) | 4, (int(rl[i]) << 4) | 3], dtype='<u4')
+            nb = nib[qo:qo + l].copy()
+            if l & 1:
+                nb = np.append(nb, 0)
+            seq = ((nb[0::2] << 4) | nb[1::2]).astype(np.uint8).tobytes()
+            p = int(s['pos'][i])
+            name = f'p{int(s["pair_id"][i]):09d}'.encode() + b'\0'
+            body = struct.pack('<iiBBHHHiiii', int(s['tid']), p, len(name), int(s['mapq'][i]),
+                               int(_reg2bin(np.array([p]), np.array([p + max(int(rl[i]), 1)]))[0]), len(cig), int(s['flag'][i]), l,
+                               int(s['mtid'][i]), int(s['mpos'][i]), int(s['isize'][i]))
+            body += name + cig.tobytes() + seq + s['qual'][qo:qo + l].tobytes() + aux
+            out.append(struct.pack('<i', len(body)) + body)
+    _write_bgzf(path, b''.join(out), level, block)
+
+
+def _take_reads_var(soa, idx):
+    """take_reads for variable-length batches (qualities / bases re-packed read by read)"""
+    n0 = len(soa['pos'])
+    out = dict(soa)
+    for k in ('pos', 'flag', 'mapq', 'l_qseq', 'n_cigar', 'mtid', 'mpos', 'isize', 'rbits', 'pair_id'):
+        out[k] = np.ascontiguousarray(soa[k][idx])
+    inv = np.full(n0 + 1, -1, dtype=np.int64)
+    inv[idx] = np.arange(len(idx), dtype=np.int64)
+    prev = soa['prev_same_name'][idx]
+    out['prev_same_name'] = np.where(prev >= 0, inv[np.where(prev >= 0, prev, n0)], -1).astype(np.int64)
+    lq = out['l_qseq'].astype(np.int64); padded = lq + (lq & 1)
+    qo = np.concatenate([[0], np.cumsum(padded)[:-1]]).astype(np.int64)
+    src = _gather_ranges(soa['qual_off'][idx], lq); dst = _gather_ranges(qo, lq)
+    qual = np.zeros(int(padded.sum()) + 2, dtype=np.uint8); qual[dst] = soa['qual'][src]
+    nib = np.zeros(len(qual), dtype=np.uint8); nib[dst] = _nibbles(soa)[src]
+    out['qual'] = qual; out['seq4'] = np.ascontiguousarray((nib[0::2] << 4) | nib[1::2])
+    out['qual_off'] = qo.astype(np.uint64)
+    out['cigar'] = np.ascontiguousarray(soa['cigar'][_gather_ranges(soa['cigar_off'][idx], out['n_cigar'])])
+    out['cigar_off'] = np.concatenate([[0], np.cumsum(out['n_cigar'].astype(np.int64))[:-1]]).astype(np.uint64)
+    out['file_start'] = np.array([0, len(idx)], dtype=np.int64)
+    return out

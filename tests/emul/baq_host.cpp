@@ -2,7 +2,8 @@
 // samtools_b200/csrc/baq_reg.h on the CPU, read by read, and compares the rewritten qualities with the oracle's
 // restatement of sam_prob_realn (oracle/baq.c, flag 3 = APPLY|EXTEND).  The device kernel executes the same
 // __host__ __device__ functions; only the memory policy differs.
-//   baq_host in.sam ref.fa   -> "checked N reads (M on the register path), K mismatches"
+//   baq_host in.sam ref.fa [-l]   -> "checked N reads (M on the register path), K mismatches"
+//   -l also lists the reads the register path takes ("reg <qname> <pos> <l_qseq>", one per line)
 // build: tests/emul/build.sh (g++ -ffp-contract=off, links oracle/_build/liboracle.so)
 #include <stdio.h>
 #include <stdlib.h>
@@ -37,9 +38,13 @@ struct HostMem {
     int32_t get_word(int j) const { return w[j]; }
 };
 
+// longest read k_baq_plan sends to the register kernel (BAQR_MAX_LQ in baq.cuh); longer band-7 reads run on k_baq
+constexpr int kMaxRegLq = 512;
+
 int main(int argc, char **argv)
 {
-    if (argc < 3) { fprintf(stderr, "usage: baq_host in.sam ref.fa\n"); return 2; }
+    if (argc < 3) { fprintf(stderr, "usage: baq_host in.sam ref.fa [-l]\n"); return 2; }
+    const bool list = argc > 3 && strcmp(argv[3], "-l") == 0;
     reader_t *rd = reader_open(argv[1], NULL);
     fasta_t *fa = fasta_load(argv[2]);
     if (!rd || !fa) { fprintf(stderr, "cannot open inputs\n"); return 2; }
@@ -86,9 +91,11 @@ int main(int argc, char **argv)
             int64_t d2 = l_ref - lq; if (d2 < 0) d2 = -d2;
             if (b2 < d2) b2 = (int)d2;
             if (b2 != baqr::BW) fast = false;
+            if (lq > kMaxRegLq) fast = false;
         }
         if (fast) {
             ++n_fast;
+            if (list) printf("reg %s %lld %d\n", r.qname, (long long)r.pos, lq);
             HostMem mem; mem.ref = ref; mem.ref_len = ref_len; mem.xb = xb;
             mem.fm.assign((size_t)(lq + 2) * baqr::NB, 0.); mem.fi = mem.fm; mem.iv.assign(lq + 2, 0.); mem.w.assign(lq + 1, 0);
             std::vector<uint8_t> q(r.qual, r.qual + lq);

@@ -11,8 +11,8 @@ import random
 OPS_REF = 'MDN=X'
 
 
-def rand_cigar(rng, max_len=40):
-    n_ops = rng.choice([1, 1, 1, 2, 3, 4, 6])
+def rand_cigar(rng, max_len=40, indel_max=6, n_ops_choices=(1, 1, 1, 2, 3, 4, 6)):
+    n_ops = rng.choice(n_ops_choices)
     ops = []
     if rng.random() < 0.15:
         ops.append((rng.randint(1, 5), 'H'))
@@ -26,7 +26,7 @@ def rand_cigar(rng, max_len=40):
             core.append((rng.randint(1, max_len), rng.choice('MMMM=X')))
         else:
             op = rng.choice('IDDNPI')
-            ln = rng.randint(1, 6) if op != 'N' else rng.randint(1, 700)
+            ln = rng.randint(1, indel_max) if op != 'N' else rng.randint(1, 700)
             core.append((ln, op))
             if rng.random() < 0.2:                    # compound: D after I, P after I, D after D ...
                 core.append((rng.randint(1, 3), rng.choice('IDP')))
@@ -42,15 +42,19 @@ def rand_cigar(rng, max_len=40):
     return ops
 
 
-def make_sam(seed, n_reads=60, n_contigs=2, contig_len=1500, with_ref=True):
+def make_sam(seed, n_reads=60, n_contigs=2, contig_len=1500, with_ref=True, long=False):
+    """long: the long-read flavour -- reads up to ~3 kb with many ops and indels up to 40 bases (BAQ bands over several
+    32-cell chunks), on 20-kb contigs"""
     rng = random.Random(seed)
+    if long:
+        contig_len = 20_000
     names = [f'c{i}' for i in range(n_contigs)]
     refs = [''.join(rng.choice('ACGTACGTACGTN' if rng.random() < 0.3 else 'ACGT') for _ in range(contig_len)) for _ in names]
     recs = []
     for i in range(n_reads):
         tid = rng.randrange(n_contigs)
         pos = rng.choice([rng.randint(1, contig_len - 50), rng.randint(1, 60), 100, 100, 101])
-        cig = rand_cigar(rng)
+        cig = rand_cigar(rng, 400, 40, (3, 5, 9, 13)) if long else rand_cigar(rng)
         qlen = sum(l for l, o in cig if o in 'MIS=X')
         rlen = sum(l for l, o in cig if o in 'MDN=X')
         flag = rng.choice([0, 16, 99, 147, 83, 163, 65, 129, 73, 1, 1024, 256, 512, 2048 + 16, 4, 99, 147])

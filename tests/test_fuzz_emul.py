@@ -12,19 +12,19 @@ def emul_bin():
     return os.path.join(ROOT, 'tests', 'emul', '_build', 'b200samtools_emul')
 
 
-def run_all(tool, oracle, td, seeds, need_noBAQ, with_gl=False):
+def run_all(tool, oracle, td, seeds, need_noBAQ, with_gl=False, long=False):
     """every (seed, command line): oracle output vs tool output; a few processes in flight (the cases are independent
     and read-only; on the GPU each tool process pays ~1 s of CUDA context creation)"""
     from concurrent.futures import ThreadPoolExecutor
     tasks = []
     for seed in seeds:
-        sam, fa = fuzz_sam.make_sam(seed)
+        sam, fa = fuzz_sam.make_sam(seed, long=long)
         d = td / f's{seed}'; d.mkdir()
         (d / 'x.sam').write_text(sam); (d / 'x.fa').write_text(fa)
         (d / 'x.bed').write_text('c0\t40\t300\nc0\t250\t600\nc1\t100\nc1\t95\t140\n')
         (d / 'rg.txt').write_text('g2\n')
         (d / 'x3.bed').write_text('#chrom\tchromStart\tchromEnd\tname\nc0\t40\t300\ta\nc1\t95\t140\tb\nc0\t250\t600\tc\nc0\t10\t10\td\nc1\t0\t2000\te\n')
-        (d / 'x2.sam').write_text(fuzz_sam.make_sam(seed + 100000, n_reads=25)[0])
+        (d / 'x2.sam').write_text(fuzz_sam.make_sam(seed + 100000, n_reads=25, long=long)[0])
         cases = [('mpileup', o) for o in fuzz_sam.MPILEUP_OPTS] + [('depth', o) for o in fuzz_sam.DEPTH_OPTS] + \
                 [('coverage', o) for o in fuzz_sam.COVERAGE_OPTS]
         cases += [('bedcov', o) for o in fuzz_sam.BEDCOV_OPTS]
