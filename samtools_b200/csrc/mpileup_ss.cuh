@@ -4,7 +4,7 @@
 // only on sums: n_plp (reads over the column), cnt (entries with base quality >= -Q) and the
 // extra bytes of special entries ("^"+mapq at a read's first column, "$" at its last, indel
 // text).  So the size pass can be read-major with no ordering constraint at all:
-//   k_mp_entries (mpileup_ent.cuh) one warp per read, lanes along the read: a coverage difference array gets
+//   k_mp_entries (mpileup_ent.cuh) one warp per 32 reads, lanes over their bases: a coverage difference array gets
 //                +1/-1 per read, only FAILING bases and special entries touch per-column counters (sparse atomics)
 //   k_ss_scan    prefix sum of the difference array -> n_plp per column
 //   k_ss_cols    per column: cnt = n_plp - fail, seq_len = cnt + extra -> MpFileSz, line length,
