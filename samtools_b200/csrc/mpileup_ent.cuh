@@ -238,12 +238,15 @@ struct MpEntFmt {
 constexpr int ENT_PAD = 64;
 
 // ---- the gather: one warp per 32-column group ------------------------------------------------------------------------
-// Two phases per chunk of 32 reads of the group's slice, with shared memory as the transpose buffer:
-//   fetch   LANES ALONG THE READS: each lane brings in the 32 entries of its read that lie over the group -- 64 contiguous
-//           bytes of the read's entry string -- with five aligned 16-byte loads (all in flight at once, no dependent chain) and
-//           parks them in its row of the warp's buffer; reads that do not reach the group get no row (ballot compaction,
-//           file order kept).  A row header carries where column c0's entry sits in the row, which columns the read covers,
-//           and its mapq / flags word.
+// The kernel issues every tile-level load (column lengths and states, the tile's output offset, the warp's read range) at
+// entry, before the block scan, so that they cost one round trip together.  Then two phases per round of 32 slice positions
+// of the group's read range, with shared memory as the transpose buffer:
+//   fetch   LANES ALONG THE READS: each lane loads its read's whole 32-byte descriptor (one sector: the second-array offset
+//           of a read with indels does not wait on its flags).  Reads that reach the group get a row (ballot compaction, file
+//           order kept); the 32 entries of a read over the group -- 64 contiguous bytes of its entry string -- go straight
+//           from global memory into its row with five aligned 16-byte cp.async copies, not through registers.  A row header
+//           carries where column c0's entry sits in the row, which columns the read covers, and its mapq / flags word.  So a
+//           round waits on two round trips (descriptors, entries), three for a group with far-reaching reads (their index list).
 //   append  LANES ALONG THE COLUMNS: the warp walks the rows in file order; lane c picks its entry out of the row with a
 //           2-byte shared-memory load (one row = 16 consecutive banks: conflict free) and appends the sequence / quality
 //           characters to its own line through cursors it keeps in registers.  No global-memory latency inside this loop,
@@ -263,44 +266,54 @@ __device__ __noinline__ SpecialEnt ent_special_g(const MpEntFmt *g, int32_t i, i
     return r;
 }
 
-constexpr int GROW = 88;                       // bytes per row: 80 fetched + 8 so that 8-byte stores of consecutive lanes hit distinct banks
+// Row buffer of a warp: one row of GROW bytes per slice position of a round.  GROW is a multiple of 16 (cp.async needs
+// 16-byte aligned destinations); with 80 = 5 x 16 the eight 16-byte copies of a quarter warp land in distinct bank groups.
+// 4 warps x 32 rows x (80 + 16 header) bytes = 12 KB per CTA; with the ~16 KB text budget at 30x / 150 bp, 7 CTAs per SM.
+constexpr int GROW = 80, GROWS = 32;
 struct GHdr { uint32_t off, vm, pk; int32_t i; };   // byte offset of column c0's entry in the warp's row buffer, columns covered, qstart|mapq|flags, read index
 
 __device__ __forceinline__ void sts8(uint32_t saddr, uint32_t v) { asm volatile("st.shared.u8 [%0], %1;" :: "r"(saddr), "r"(v) : "memory"); }
 
-// what one lane brings in for its read of a chunk: 80 bytes of the read's entry string around column c0 + the row header fields
-struct GFetch { uint4 A0, A1, A2, A3, A4; uint32_t vm, pk, o; int32_t i; };
+// one slice position of a round: the aligned start of the read's 80 bytes of entry string around column c0 + the row
+// header fields; vm == 0: the read does not reach the group (or t is past the range)
+struct GRead { const uint4 *q; uint32_t vm, pk, o; int32_t i; };
 
-__device__ __forceinline__ GFetch gather_fetch(const MpEntFmt &fmt, const ReadRange &rr, int32_t c0, int32_t t0)
+__device__ __forceinline__ GRead gather_read(const MpEntFmt &fmt, const ReadRange &rr, int32_t c0, int32_t t)
 {
-    const int lane = threadIdx.x & 31;
-    const View &v = fmt.v;
     const uint32_t kSimple = (uint32_t)RD_SIMPLE << 24;
-    GFetch f;
-    f.A0 = f.A1 = f.A2 = f.A3 = f.A4 = make_uint4(0u, 0u, 0u, 0u);
-    f.vm = 0; f.pk = 0; f.o = 0; f.i = 0;
-    const int32_t t = t0 + lane;
+    GRead f;
+    f.q = nullptr; f.vm = 0; f.pk = 0; f.o = 0; f.i = 0;
     if (t < rr.n) {
         f.i = range_at(rr, t);
-        const uint4 d = __ldg(reinterpret_cast<const uint4 *>(v.desc + f.i));
+        const uint4 *dp = reinterpret_cast<const uint4 *>(fmt.v.desc + f.i);
+        const uint4 d = __ldg(dp), d2 = __ldg(dp + 1);       // hot and cold half of the descriptor: one 32-byte sector
         const int32_t rpos = (int32_t)d.x, rend = (int32_t)d.y;
         f.pk = d.w;
         const int32_t lo_c = rpos > c0 ? rpos - c0 : 0, hi_c = rend - c0 < 32 ? rend - c0 : 32;
         if (hi_c > lo_c) {
             f.vm = (hi_c >= 32 ? 0xffffffffu : (1u << hi_c) - 1u) & ~((1u << lo_c) - 1u);
-            const uint16_t *src = (f.pk & kSimple) ? fmt.E + (d.z + (f.pk & 0xffffu)) : fmt.E2 + __ldg(&v.desc[f.i].pad_);
+            const uint16_t *src = (f.pk & kSimple) ? fmt.E + (d.z + (f.pk & 0xffffu)) : fmt.E2 + d2.w;   // d2.w: pad_
             src += c0 - rpos;                                  // entry of column c0 (before the read's first entry when the read starts inside the group)
             const unsigned long long a = (unsigned long long)src;
-            const uint4 *q = reinterpret_cast<const uint4 *>(a & ~15ull);
+            f.q = reinterpret_cast<const uint4 *>(a & ~15ull);
             f.o = (uint32_t)(a & 15ull);                       // bytes between the aligned address and column c0's entry
-            f.A0 = __ldg(q); f.A1 = __ldg(q + 1); f.A2 = __ldg(q + 2); f.A3 = __ldg(q + 3); f.A4 = __ldg(q + 4);
         }
     }
     return f;
 }
 
+// row `row` of the warp's buffer: the read's 80 bytes through cp.async (in flight until the caller's wait), then its header
+__device__ __forceinline__ void gather_row(uint32_t rows_s, GHdr *hdr, uint32_t row, const GRead &f)
+{
+    const uint32_t s = rows_s + row * GROW;
+#pragma unroll
+    for (int k = 0; k < GROW / 16; ++k) asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(s + 16u * k), "l"(f.q + k) : "memory");
+    GHdr h; h.off = row * GROW + f.o; h.vm = f.vm; h.pk = f.pk; h.i = f.i;
+    *reinterpret_cast<uint4 *>(hdr + row) = *reinterpret_cast<const uint4 *>(&h);
+}
+
 template <bool OUT_MAPQ>
-__device__ __forceinline__ void gather_group(const MpEntFmt &fmt, const MpEntFmt *gfmt, int32_t c0, bool on,
+__device__ __forceinline__ void gather_group(const MpEntFmt &fmt, const MpEntFmt *gfmt, const ReadRange &rr, int32_t c0, bool on,
                                              uint32_t so, uint32_t qo, uint32_t mo, char *sb, unsigned char *rows, GHdr *hdr)
 {
     const uint32_t sb_s = (uint32_t)__cvta_generic_to_shared(sb);
@@ -308,27 +321,20 @@ __device__ __forceinline__ void gather_group(const MpEntFmt &fmt, const MpEntFmt
     const int lane = threadIdx.x & 31;
     const uint32_t lt = (1u << lane) - 1u;
     const int32_t c = c0 + lane;
-    const ReadRange rr = read_range(fmt.v, 0, c0 >> 5);            // the same for the 32 lanes
-    for (int32_t t0 = 0; t0 < rr.n; t0 += 32) {
-        const GFetch f = gather_fetch(fmt, rr, c0, t0);
-        // ---- rows of this chunk: lane = read
+    const uint32_t rows_base = (uint32_t)__cvta_generic_to_shared(rows);
+    for (int32_t t0 = 0; t0 < rr.n; t0 += GROWS) {
+        const GRead f = gather_read(fmt, rr, c0, t0 + lane);
+        // ---- rows of this round: lane = read
         const uint32_t live = __ballot_sync(0xffffffffu, f.vm != 0u);
         if (!live) continue;
-        __syncwarp();                                              // the previous chunk's rows have been consumed
-        if (f.vm) {
-            const uint32_t row = (uint32_t)__popc(live & lt);
-            uint2 *w = reinterpret_cast<uint2 *>(rows + row * GROW);
-            w[0] = make_uint2(f.A0.x, f.A0.y); w[1] = make_uint2(f.A0.z, f.A0.w); w[2] = make_uint2(f.A1.x, f.A1.y); w[3] = make_uint2(f.A1.z, f.A1.w);
-            w[4] = make_uint2(f.A2.x, f.A2.y); w[5] = make_uint2(f.A2.z, f.A2.w); w[6] = make_uint2(f.A3.x, f.A3.y); w[7] = make_uint2(f.A3.z, f.A3.w);
-            w[8] = make_uint2(f.A4.x, f.A4.y); w[9] = make_uint2(f.A4.z, f.A4.w);
-            GHdr h; h.off = row * GROW + f.o; h.vm = f.vm; h.pk = f.pk; h.i = f.i;
-            *reinterpret_cast<uint4 *>(hdr + row) = *reinterpret_cast<const uint4 *>(&h);
-        }
-        __syncwarp();
+        __syncwarp();                                              // the previous round's rows have been consumed
+        if (f.vm) gather_row(rows_base, hdr, (uint32_t)__popc(live & lt), f);
+        asm volatile("cp.async.wait_all;" ::: "memory");           // this lane's copies have landed ...
+        __syncwarp();                                              // ... and every lane's: the rows are complete
         // ---- append: lane = column (cursors are 32-bit shared-memory addresses: plain st.shared, no generic-address arithmetic)
         const int nrows = __popc(live);
         if (on) {
-            const uint32_t rows_s = (uint32_t)__cvta_generic_to_shared(rows) + 2u * (uint32_t)lane;
+            const uint32_t rows_s = rows_base + 2u * (uint32_t)lane;
             for (int r = 0; r < nrows; ++r) {
                 const uint4 hw = *reinterpret_cast<const uint4 *>(hdr + r);          // broadcast
                 uint32_t e;
@@ -364,23 +370,27 @@ __global__ void __launch_bounds__(TILE, MIN_CTAS) k_mp_gather(MpEntFmt fmt, cons
 {
     extern __shared__ __align__(16) char s_text[];
     __shared__ uint32_t s_ws[TILE / 32];
-    __shared__ __align__(16) unsigned char s_rows[TILE / 32][32 * GROW];
-    __shared__ __align__(16) GHdr s_hdr[TILE / 32][32];
+    __shared__ __align__(16) unsigned char s_rows[TILE / 32][GROWS * GROW];
+    __shared__ __align__(16) GHdr s_hdr[TILE / 32][GROWS];
     const int32_t ncols = fmt.v.ncols;
     const int32_t c = (int32_t)blockIdx.x * TILE + (int32_t)threadIdx.x;
-    MpFileSz stt;
-    uint32_t len = 0;
-    if (c < ncols) { len = len_in[c]; if (len) stt = st_in[c]; }
+    const int32_t c0 = (int32_t)(blockIdx.x * TILE + (threadIdx.x & ~31u));
+    // Every tile-level load goes out here, unconditionally and before the block scan, so that they share one round trip:
+    // the column's length and state (both arrays cover the whole last tile; beyond ncols the length is not written and
+    // is replaced by 0), the tile's output offset, and the warp's read range (a warp past the window reads the last group's).
+    uint32_t len = len_in[c];
+    const MpFileSz stt = st_in[c];
+    if (c >= ncols) len = 0;
+    const uint64_t base = tile_base[blockIdx.x];
+    const ReadRange rr = read_range(fmt.v, 0, min(c0 >> 5, fmt.v.n_tiles - 1));   // the same for the 32 lanes
     uint32_t total;
     const uint32_t off = block_excl_scan<TILE>(len, s_ws, total);
     if (total == 0) return;
-    const uint64_t base = tile_base[blockIdx.x];
     const uint32_t phase = (uint32_t)(base & 15);
     if (total + phase <= smem_cap) {
         char *sb = s_text + phase;
         // every line's fixed parts (header, count, separators, place holders, newline) by the column's own thread ...
         const int wi = threadIdx.x >> 5, lane = threadIdx.x & 31;
-        const int32_t c0 = (int32_t)(blockIdx.x * TILE + (threadIdx.x & ~31u));
         uint32_t so = 0, qo = 0, mo = 0;
         bool on = false;
         if (len) {
@@ -388,7 +398,7 @@ __global__ void __launch_bounds__(TILE, MIN_CTAS) k_mp_gather(MpEntFmt fmt, cons
             if (k.ps) { on = true; so = (uint32_t)(k.ps - sb); qo = (uint32_t)(k.pq - sb); mo = OUT_MAPQ ? (uint32_t)(k.pm - sb) : 0u; }
         }
         // ... then the entries of the warp's 32 columns
-        if (__any_sync(0xffffffffu, on)) gather_group<OUT_MAPQ>(fmt, gfmt, c0, on, so, qo, mo, sb, s_rows[wi], s_hdr[wi]);
+        if (__any_sync(0xffffffffu, on)) gather_group<OUT_MAPQ>(fmt, gfmt, rr, c0, on, so, qo, mo, sb, s_rows[wi], s_hdr[wi]);
         // Each warp stores its own 32 lines (contiguous in the tile) as soon as it has them: no block-wide barrier at the end,
         // so a warp with a deep column does not hold the other three.  Ragged head (to the next 16 B boundary of the
         // destination) and tail by the lanes, the aligned body through one TMA bulk store (shared memory is laid out with the
