@@ -93,6 +93,12 @@ typedef struct {
 #define B200_RB_HALO      8   /* the read starts before this window and was already staged with the previous one (a driver that
                                  cuts a reference sequence into column windows stages every read overlapping a window: the -r
                                  rule, bam_plcmd.c:550-554,609): leave it out of the coverage read statistics (coverage.c:185-193) */
+/* The max-depth rule of bam_plp_push depends on every read pushed before: a driver that cuts a reference sequence into
+ * windows stages the reads that reach a window from the left again and hands over the verdicts the previous window made
+ * (b200_fetch_mapq_keep: 2 = kept, 3 = dropped).  A SEEN read is not judged again: kept, it counts as buffered and as the
+ * previous read; dropped, it takes no part.  Only reads without SEEN are judged. */
+#define B200_RB_MAXDEPTH_SEEN 16   /* the read's max-depth verdict was made in an earlier window */
+#define B200_RB_MAXDEPTH_DROP 32   /* ... and that verdict was a drop */
 
 /* ---- read-level configuration (what happens before a read is pushed) ---- */
 typedef enum { B200_MODE_MPILEUP = 0, B200_MODE_DEPTH = 1, B200_MODE_COVERAGE = 2 } b200_mode_t;

@@ -710,13 +710,15 @@ static int max_buffered_reads(b200_engine *e, int *out)
 }
 
 // max-depth rule of bam_plp_push, evaluated on the host only when a column could
-// hold more than maxcnt reads (sequential by nature; see DESIGN.md).
+// hold more than maxcnt reads (sequential by nature; see DESIGN.md).  Reads whose verdict an earlier window made
+// (B200_RB_MAXDEPTH_SEEN) are not judged again: the kept ones only fill the buffer, the dropped ones are ST_MAXDROP already.
 static int apply_maxcnt_host(b200_engine *e, int64_t n, int maxcnt)
 {
     std::vector<ReadDesc> hd((size_t)n);
-    std::vector<uint8_t> st((size_t)n);
+    std::vector<uint8_t> st((size_t)n), rb;
     CK(cudaMemcpyAsync(hd.data(), e->desc, (size_t)n * sizeof(ReadDesc), cudaMemcpyDeviceToHost, e->stream));
     CK(cudaMemcpyAsync(st.data(), e->state, (size_t)n, cudaMemcpyDeviceToHost, e->stream));
+    if (e->has_rbits) { rb.resize((size_t)n); CK(cudaMemcpyAsync(rb.data(), e->rbits, (size_t)n, cudaMemcpyDeviceToHost, e->stream)); }
     CK(cudaStreamSynchronize(e->stream));
     bool changed = false;
     for (int f = 0; f < e->n_files; ++f) {
@@ -725,7 +727,7 @@ static int apply_maxcnt_host(b200_engine *e, int64_t n, int maxcnt)
         for (int64_t i = e->h_file_start[f]; i < e->h_file_start[f + 1]; ++i) {
             if (st[i] != ST_KEEP) continue;
             const int32_t pos = hd[i].rpos, end = hd[i].rpos + e->h_rlen_tmp[i];
-            if (have_prev) {
+            if (have_prev && !(e->has_rbits && (rb[i] & B200_RB_MAXDEPTH_SEEN))) {
                 while (!ends.empty() && ends.top() < p_prev) ends.pop();   // buffered = accepted reads with end >= previous accepted start
                 if (pos == p_prev && (int64_t)ends.size() + 1 > (int64_t)maxcnt) { st[i] = ST_MAXDROP; changed = true; continue; }
             }

@@ -26,6 +26,7 @@
 #include <cerrno>
 #include <algorithm>
 #include <thread>
+#include <queue>
 #include <set>
 #include <unordered_map>
 
@@ -152,21 +153,71 @@ int run_window_rounds(std::vector<std::unique_ptr<WinWorker>> &workers, const st
 // stages every record that overlaps it -- pos < we && endpos > wb, the rule a `-r` run applies (bam_plcmd.c:550-554,609)
 // -- so a read reaching in from the left is staged again ("halo"); the engine reports only columns inside the window.
 // Per-read work (filters, BAQ) is simply repeated for halo reads; a mate pair whose overlap lies in the window has both
-// mates staged, so the overlap tweak sees what an unsplit run sees.  NOT carried across a window edge: the buffer
-// occupancy the -d max-depth rule of bam_plp_push looks at (only matters when a column holds more reads than -d).
+// mates staged, so the overlap tweak sees what an unsplit run sees.  The -d max-depth rule of bam_plp_push counts a read
+// as buffered over the closed interval [pos, endpos], so a window that continues an earlier one also stages the reads
+// ending right at its start (endpos == wb: they cover none of its columns), and the halo reads carry the verdicts the
+// earlier window made (B200_RB_MAXDEPTH_*; see MaxDepthCarry).
 int64_t window_cols()
 {
     static int64_t w = 0;
     if (!w) { const char *s = getenv("B200_WINDOW_COLS"); w = s ? atoll(s) : (1LL << 24); if (w < 1) w = 1; if (w > (1LL << 30)) w = 1LL << 30; }
     return w;
 }
-// records of v (sorted by pos) overlapping [wb,we); `lo` is a cursor that only moves forward across successive windows
-void window_records(const std::vector<Record> &v, size_t &lo, int64_t wb, int64_t we, std::vector<size_t> &out)
+// records of v (sorted by pos) overlapping [wb,we) -- with `closed`, also those ending at wb; `lo` is a cursor that only
+// moves forward across successive windows
+void window_records(const std::vector<Record> &v, size_t &lo, int64_t wb, int64_t we, std::vector<size_t> &out, bool closed = false)
 {
     out.clear();
-    while (lo < v.size() && v[lo].endpos() <= wb) ++lo;
-    for (size_t j = lo; j < v.size() && v[j].pos < we; ++j) if (v[j].endpos() > wb) out.push_back(j);
+    const int64_t lim = closed && wb > INT64_MIN ? wb - 1 : wb;
+    while (lo < v.size() && v[lo].endpos() <= lim) ++lo;
+    for (size_t j = lo; j < v.size() && v[j].pos < we; ++j) if (v[j].endpos() > lim) out.push_back(j);
 }
+// Largest number of records of one file (before any filter) whose closed intervals [pos, endpos] share a position: no
+// column of the contig can make the max-depth rule fire while this is <= -d, and then its windows are independent.
+int64_t max_stacked_records(const std::vector<FileData> &fd, int tid)
+{
+    int64_t best = 0;
+    for (const FileData &f : fd) {
+        if (tid >= (int)f.by_tid.size()) continue;
+        std::priority_queue<int64_t, std::vector<int64_t>, std::greater<int64_t>> ends;
+        int64_t last = INT64_MIN;
+        for (const Record &r : f.by_tid[(size_t)tid]) {
+            if (r.pos < last) return INT64_MAX;   // unsorted: the engine refuses it; no bound
+            last = r.pos;
+            while (!ends.empty() && ends.top() < r.pos) ends.pop();
+            ends.push(r.endpos());
+            if ((int64_t)ends.size() > best) best = (int64_t)ends.size();
+        }
+    }
+    return best;
+}
+// The max-depth verdicts of one contig's records, handed from each window to the next: after a window is staged, every
+// record the engine kept (2) or dropped (3) remembers it, and a later window that stages the record again passes it on.
+struct MaxDepthCarry {
+    bool on = false;
+    std::vector<std::vector<uint8_t>> bits;   // per file, per record of the contig: B200_RB_MAXDEPTH_* or 0
+    std::vector<std::pair<int, size_t>> staged;   // (file, record) of each read of the staged batch
+    std::vector<uint8_t> keep;
+    void reset(const std::vector<FileData> &fd, int tid, bool enable)
+    {
+        on = enable; bits.assign(fd.size(), {}); staged.clear();
+        if (on) for (size_t i = 0; i < fd.size(); ++i) bits[i].assign(tid < (int)fd[i].by_tid.size() ? fd[i].by_tid[(size_t)tid].size() : 0, 0);
+    }
+    uint8_t add(int file, size_t j) { if (!on) return 0; staged.emplace_back(file, j); return bits[(size_t)file][j]; }
+    int collect(b200_engine_t *e)
+    {
+        if (!on) return 0;
+        keep.resize(staged.size());
+        if (!staged.empty() && b200_fetch_mapq_keep(e, nullptr, keep.data(), keep.size()) != 0) return -1;
+        for (size_t k = 0; k < staged.size(); ++k) {
+            uint8_t &b = bits[(size_t)staged[k].first][staged[k].second];
+            if (keep[k] == 2) b = B200_RB_MAXDEPTH_SEEN;
+            else if (keep[k] == 3) b = B200_RB_MAXDEPTH_SEEN | B200_RB_MAXDEPTH_DROP;
+        }
+        staged.clear();
+        return 0;
+    }
+};
 // first / one-past-last reference position touched by the records of a contig (over all files)
 bool records_extent(const std::vector<FileData> &fd, int tid, int64_t &first, int64_t &last)
 {
@@ -336,22 +387,24 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn)
         for (size_t k = 0; k < nx; ++k) mc.x_sep[k] = (int)k < o.n_xfields ? ',' : o.x_sep;
         return 0;
     };
-    // one window [wb,we) of contig tid: stage the overlapping records, return the stage statistics
-    auto stage_window = [&](int tid, bool with_reads, int64_t wb, int64_t we, const std::string *ref, b200_stage_stats_t &st) -> int {
+    MaxDepthCarry md;
+    // one window [wb,we) of contig tid (cont: it continues an earlier window): stage the overlapping records, return the
+    // stage statistics
+    auto stage_window = [&](int tid, bool with_reads, int64_t wb, int64_t we, bool cont, const std::string *ref, b200_stage_stats_t &st) -> int {
         const std::string &name = h.names[(size_t)tid];
         pb.clear(); staged.clear();
         for (int i = 0; i < nfn; ++i) {
             pb.begin_file();
             if (with_reads && tid < (int)fd[(size_t)i].by_tid.size()) {
                 std::vector<Record> &v = fd[(size_t)i].by_tid[(size_t)tid];
-                window_records(v, cursor[(size_t)i], wb, we, sel);
-                for (size_t j : sel) { pb.add(v[j], hbits[(size_t)i][j], o.overlaps); if (!o.xcols.empty()) staged.push_back(&v[j]); }
+                window_records(v, cursor[(size_t)i], wb, we, sel, cont);
+                for (size_t j : sel) { pb.add(v[j], (uint8_t)(hbits[(size_t)i][j] | md.add(i, j)), o.overlaps); if (!o.xcols.empty()) staged.push_back(&v[j]); }
             }
         }
         pb.finish();
         b200_batch_t batch = pb.view(tid, h.lens[(size_t)tid], name, ref);
         sc.beg = wb; sc.end = we;
-        if (b200_stage(eng.e, &batch, &sc, &st) != 0) { fprintf(stderr, "samtools mpileup: %s\n", b200_last_error(eng.e)); return -1; }
+        if (b200_stage(eng.e, &batch, &sc, &st) != 0 || md.collect(eng.e) != 0) { fprintf(stderr, "samtools mpileup: %s\n", b200_last_error(eng.e)); return -1; }
         return 0;
     };
     auto process_tid = [&](int tid, bool with_reads) -> int {
@@ -376,16 +429,20 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn)
         // the first window with a pileup column decides whether the contig is reported at all (its empty -a rows before that
         // column included), so find it before anything is written
         int64_t first_hit = -1;
+        md.reset(fd, tid, false);
         if (with_reads) {
             std::fill(cursor.begin(), cursor.end(), 0);
             for (int64_t wb = lo_col; wb < hi_col; wb += W) {
                 b200_stage_stats_t st;
-                if (stage_window(tid, true, wb, std::min(wb + W, hi_col), ref, st) != 0) return -1;
+                if (stage_window(tid, true, wb, std::min(wb + W, hi_col), wb > lo_col, ref, st) != 0) return -1;
                 if (st.n_kept_in_window > 0) { first_hit = wb; break; }
             }
             if (first_hit < 0) return 0;
         }
-        if (with_reads && !workers.empty()) {
+        // a contig split into several windows where the max-depth rule may fire runs them in order, each handing its
+        // verdicts to the next; elsewhere the windows are independent
+        const bool carry = with_reads && hi_col - lo_col > W && max_stacked_records(fd, tid) > (int64_t)max_depth;
+        if (with_reads && !workers.empty() && !carry) {
             std::vector<std::pair<int64_t, int64_t>> wins;
             for (int64_t wb = lo_col; wb < hi_col; wb += W) wins.emplace_back(wb, std::min(wb + W, hi_col));
             const int rc = run_window_rounds(workers, wins, fp, "mpileup", [&](WinWorker &w, int64_t wb, int64_t we) {
@@ -394,7 +451,7 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn)
                     w.pb.begin_file();
                     if (tid < (int)fd[(size_t)i].by_tid.size()) {
                         std::vector<Record> &v = fd[(size_t)i].by_tid[(size_t)tid];
-                        window_records(v, w.cursor[(size_t)i], wb, we, w.sel);
+                        window_records(v, w.cursor[(size_t)i], wb, we, w.sel, wb > lo_col);
                         for (size_t j : w.sel) w.pb.add(v[j], hbits[(size_t)i][j], o.overlaps);
                     }
                 }
@@ -412,10 +469,11 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn)
             return 1;
         }
         std::fill(cursor.begin(), cursor.end(), 0);
+        md.reset(fd, tid, carry);
         for (int64_t wb = lo_col; wb < hi_col || (!with_reads && wb == lo_col); wb += W) {
             const int64_t we = std::max(std::min(wb + W, hi_col), wb);
             b200_stage_stats_t st;
-            if (stage_window(tid, with_reads, wb, we, ref, st) != 0) return -1;
+            if (stage_window(tid, with_reads, wb, we, wb > lo_col, ref, st) != 0) return -1;
             if (with_reads && !o.all && st.n_kept_in_window == 0) continue;
             if (o.gl) {
                 int64_t ncols = 0; const size_t cap = (size_t)st.n_cols + 16;
@@ -859,8 +917,12 @@ int main_coverage(int argc, char **argv)
         // column windows of [rw.beg, rw.end): the sums add up.  Every record is counted once in the read statistics
         // (coverage.c:185-193): a read that reaches in from the previous window is staged again as halo (B200_RB_HALO);
         // the first / last window also take the records that lie before / beyond the region.
+        // A window that continues an earlier one also stages the records ending right at its start (the closed intervals
+        // of the -d rule; they cover none of its columns), and where the rule may fire the windows hand their verdicts on.
         const int64_t W = window_cols();
         std::vector<size_t> sel, cursor((size_t)nfn, 0);
+        MaxDepthCarry md;
+        md.reset(fd, tid, rw.end - rw.beg > W && max_stacked_records(fd, tid) > (int64_t)sc.max_depth);
         for (int64_t wb = rw.beg; wb < rw.end || wb == rw.beg; wb += W) {
             const bool first_w = wb == rw.beg, last_w = wb + W >= rw.end;
             const int64_t we = last_w ? std::max(rw.end, wb) : wb + W;
@@ -869,15 +931,15 @@ int main_coverage(int argc, char **argv)
                 pb.begin_file();
                 if (tid >= (int)fd[(size_t)i].by_tid.size()) continue;
                 std::vector<Record> &v = fd[(size_t)i].by_tid[(size_t)tid];
-                window_records(v, cursor[(size_t)i], first_w ? INT64_MIN : wb, last_w ? POS_MAX : we, sel);
-                for (size_t j : sel) pb.add(v[j], (uint8_t)((!first_w && v[j].pos < wb) ? B200_RB_HALO : 0), false);
+                window_records(v, cursor[(size_t)i], first_w ? INT64_MIN : wb, last_w ? POS_MAX : we, sel, !first_w);
+                for (size_t j : sel) pb.add(v[j], (uint8_t)(((!first_w && v[j].pos < wb) ? B200_RB_HALO : 0) | md.add(i, j)), false);
             }
             pb.finish();
-            if (pb.pos.empty()) { if (last_w) break; continue; }
+            if (pb.pos.empty()) { md.staged.clear(); if (last_w) break; continue; }
             b200_batch_t batch = pb.view(tid, h.lens[(size_t)tid], h.names[(size_t)tid], nullptr);
             sc.beg = wb; sc.end = we;
             b200_stage_stats_t st;
-            if (b200_stage(eng.e, &batch, &sc, &st) != 0) { fprintf(stderr, "samtools coverage: %s\n", b200_last_error(eng.e)); return 1; }
+            if (b200_stage(eng.e, &batch, &sc, &st) != 0 || md.collect(eng.e) != 0) { fprintf(stderr, "samtools coverage: %s\n", b200_last_error(eng.e)); return 1; }
             rw.n_sel += st.n_selected_reads; rw.sum_mq += st.summed_mapq; rw.n_reads += st.n_reads;
             // a column exists as soon as one kept read has a non-empty reference span (before the region test)
             if (st.n_kept > 0) {

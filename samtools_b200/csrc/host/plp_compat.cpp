@@ -7,8 +7,9 @@
 // bases) -- then packed into the SoA batch image and staged, and the device returns every (read, column) entry -- the
 // bam_pileup1_t fields -- column-major; next()/auto() walk that table.  A window cut inside a reference sequence ends at
 // the start of the read that triggered it: every read that starts before it is in hand, so all columns below the cut can be
-// served; the reads reaching beyond the cut stay (the halo, exactly the -r rule of bam_plcmd.c:550-554) and are staged again
-// with the next window, which reports only columns from the cut on.  Host memory is bounded by the budget, and a push /
+// served; the reads reaching the cut stay (the halo: the -r rule of bam_plcmd.c:550-554, plus the reads ending right at the
+// cut, which the max-depth rule still counts as buffered there) and are staged again with the next window, which reports
+// only columns from the cut on and does not judge the halo reads' max-depth verdicts again (B200_RB_MAXDEPTH_*).  Host memory is bounded by the budget, and a push /
 // next client sees columns long before the reference sequence ends.  With overlaps enabled the tweaked qualities are copied back into the
 // iterator's read copies, which is what the caller sees through plp[i].b, as in htslib.
 #include "../../../include/b200_htslib_compat.h"
@@ -77,6 +78,7 @@ struct b200_plp {
     int64_t next_beg = -1;                 // where the next window of the current reference sequence starts (-1: at its first read)
     size_t accum_bytes = 0, budget = (size_t)256 << 20;
     std::vector<uint8_t> accum_done, batch_done;   // read's pair overlap was already tweaked in an earlier window (halo reads)
+    std::vector<uint8_t> accum_md, batch_md;       // max-depth verdict of an earlier window (B200_RB_MAXDEPTH_*; halo reads)
     std::vector<bam_pileup_cd> accum_cd, batch_cd; bam_pileup_cd pending_cd;   // client data of the same reads
     bam_plp_cd_f construct = nullptr, destruct = nullptr;
     int last_tid = -1; hts_pos_t last_pos = -1;
@@ -133,6 +135,7 @@ static int stage_batch(b200_plp *it)
             if (f != names.end()) { pv = f->second; f->second = (int64_t)i; } else names.emplace(qn, (int64_t)i);
             if (name_bit(qn)) rb |= B200_RB_NAME_ODD;
         }
+        rb |= it->batch_md[i];
         it->prev.push_back(pv); it->rbits.push_back(rb);
     }
     if (it->seq4.size() * 2 < it->qual.size() + 2) it->seq4.resize((it->qual.size() + 2) / 2, 0);
@@ -157,6 +160,13 @@ static int stage_batch(b200_plp *it)
         for (size_t i = 0; i < n; ++i) memcpy(bam_get_qual(it->batch[i]), q.data() + it->qual_off[i], (size_t)it->batch[i]->core.l_qseq);
         // both mates staged together -> their tweak has happened (and is now in the copies): not again in a later window
         for (size_t i = 0; i < n; ++i) if (it->prev[i] >= 0) { it->batch_done[i] = 1; it->batch_done[(size_t)it->prev[i]] = 1; }
+    }
+    if (it->serve_end < kPosMax && it->maxcnt > 0) {   // the halo reads take this window's max-depth verdicts to the next one
+        std::vector<uint8_t> keep(n);
+        if (b200_fetch_mapq_keep(it->eng, nullptr, keep.data(), n) != 0) return -1;
+        for (size_t i = 0; i < n; ++i)
+            if (keep[i] == 2) it->batch_md[i] = B200_RB_MAXDEPTH_SEEN;
+            else if (keep[i] == 3) it->batch_md[i] = B200_RB_MAXDEPTH_SEEN | B200_RB_MAXDEPTH_DROP;
     }
     it->col = 0; it->slab_beg = it->slab_end = 0; it->ent_pos = 0;
     return 0;
@@ -188,18 +198,22 @@ static const bam_pileup1_t *serve(b200_plp *it, int *_tid, hts_pos_t *_pos, int 
         if (it->col >= it->n_cols) {
             it->serving = false;
             if (it->serve_end < kPosMax) {
-                // window cut inside the reference sequence: reads reaching beyond the cut go back to the front of the collection
-                std::vector<bam1_t *> keep; std::vector<bam_pileup_cd> keep_cd; std::vector<uint8_t> keep_done; size_t bytes = 0;
+                // window cut inside the reference sequence: reads reaching the cut go back to the front of the collection --
+                // those ending right at it too, as the max-depth rule still counts them as buffered there
+                std::vector<bam1_t *> keep; std::vector<bam_pileup_cd> keep_cd; std::vector<uint8_t> keep_done, keep_md; size_t bytes = 0;
                 for (size_t i = 0; i < it->batch.size(); ++i) {
                     bam1_t *b = it->batch[i];
-                    if (read_end(b) > it->serve_end) { keep.push_back(b); keep_cd.push_back(it->batch_cd[i]); keep_done.push_back(it->batch_done[i]); bytes += (size_t)b->core.l_qseq; }
-                    else { if (it->destruct) it->destruct(it->data, b, &it->batch_cd[i]); bam_destroy1(b); }
+                    if (read_end(b) >= it->serve_end) {
+                        keep.push_back(b); keep_cd.push_back(it->batch_cd[i]); keep_done.push_back(it->batch_done[i]); keep_md.push_back(it->batch_md[i]);
+                        bytes += (size_t)b->core.l_qseq;
+                    } else { if (it->destruct) it->destruct(it->data, b, &it->batch_cd[i]); bam_destroy1(b); }
                 }
-                it->batch.clear(); it->batch_cd.clear(); it->batch_done.clear();
+                it->batch.clear(); it->batch_cd.clear(); it->batch_done.clear(); it->batch_md.clear();
                 keep.insert(keep.end(), it->accum.begin(), it->accum.end()); keep_cd.insert(keep_cd.end(), it->accum_cd.begin(), it->accum_cd.end());
                 keep_done.insert(keep_done.end(), it->accum_done.begin(), it->accum_done.end());
-                it->accum.swap(keep); it->accum_cd.swap(keep_cd); it->accum_done.swap(keep_done); it->accum_bytes += bytes;
-            } else { free_reads(it, it->batch, it->batch_cd); it->batch_done.clear(); }
+                keep_md.insert(keep_md.end(), it->accum_md.begin(), it->accum_md.end());
+                it->accum.swap(keep); it->accum_cd.swap(keep_cd); it->accum_done.swap(keep_done); it->accum_md.swap(keep_md); it->accum_bytes += bytes;
+            } else { free_reads(it, it->batch, it->batch_cd); it->batch_done.clear(); it->batch_md.clear(); }
             break;
         }
         if (it->col >= it->slab_end) { if (load_slab(it) != 0) { it->error = true; *_n = -1; return nullptr; } }
@@ -226,8 +240,8 @@ static const bam_pileup1_t *serve(b200_plp *it, int *_tid, hts_pos_t *_pos, int 
 // the collected contig becomes the served one
 static int start_serving(b200_plp *it)
 {
-    it->batch.swap(it->accum); it->batch_cd.swap(it->accum_cd); it->batch_done.swap(it->accum_done);
-    it->accum.clear(); it->accum_cd.clear(); it->accum_done.clear(); it->accum_bytes = 0;
+    it->batch.swap(it->accum); it->batch_cd.swap(it->accum_cd); it->batch_done.swap(it->accum_done); it->batch_md.swap(it->accum_md);
+    it->accum.clear(); it->accum_cd.clear(); it->accum_done.clear(); it->accum_md.clear(); it->accum_bytes = 0;
     if (it->batch.empty()) return 0;
     it->tid = it->batch[0]->core.tid;
     // the previous window of this reference sequence ended at next_beg; this one ends at the start of the read that cut it
@@ -268,7 +282,7 @@ void bam_plp_reset(bam_plp_t it)
     free_pending(it);
     it->serving = false; it->eof = false; it->error = false; it->last_tid = -1; it->last_pos = -1;
     it->cut = false; it->serve_beg = -1; it->serve_end = kPosMax; it->next_beg = -1; it->accum_bytes = 0;
-    it->accum_done.clear(); it->batch_done.clear();
+    it->accum_done.clear(); it->batch_done.clear(); it->accum_md.clear(); it->batch_md.clear();
 }
 
 void bam_plp_set_maxcnt(bam_plp_t it, int maxcnt) { it->maxcnt = maxcnt; }
@@ -301,7 +315,7 @@ int bam_plp_push(bam_plp_t it, const bam1_t *b)
         it->pending = c; it->pending_cd = cd; it->cut = over;
     } else {
         if (it->construct) it->construct(it->data, c, &cd);
-        it->accum.push_back(c); it->accum_cd.push_back(cd); it->accum_done.push_back(0); it->accum_bytes += (size_t)c->core.l_qseq;
+        it->accum.push_back(c); it->accum_cd.push_back(cd); it->accum_done.push_back(0); it->accum_md.push_back(0); it->accum_bytes += (size_t)c->core.l_qseq;
     }
     return 0;
 }
@@ -317,7 +331,7 @@ const bam_pileup1_t *bam_plp64_next(bam_plp_t it, int *_tid, hts_pos_t *_pos, in
         if (it->pending || (it->eof && !it->accum.empty())) {
             if (start_serving(it) != 0) { *_n = -1; return nullptr; }
             if (it->pending) {
-                it->accum.push_back(it->pending); it->accum_cd.push_back(it->pending_cd); it->accum_done.push_back(0);
+                it->accum.push_back(it->pending); it->accum_cd.push_back(it->pending_cd); it->accum_done.push_back(0); it->accum_md.push_back(0);
                 it->accum_bytes += (size_t)it->pending->core.l_qseq; it->pending = nullptr; it->cut = false;
             }
             continue;

@@ -159,6 +159,8 @@ PLP_HD void stage_prep2(const RawSoA &r, const b200_stage_conf_t &cf, int64_t i,
         if (r.mapq[i] < cf.min_mq) keep = false;
         else if (cf.no_orphan && (fl & 1) && !(fl & 2)) keep = false;
     }
+    // a drop decided by the max-depth rule in an earlier window holds even where this window alone could not fire the rule
+    if (keep && cf.mode != B200_MODE_DEPTH && cf.max_depth > 0 && r.rbits && (r.rbits[i] & B200_RB_MAXDEPTH_DROP)) { state[i] = ST_MAXDROP; return; }
     state[i] = keep ? ST_KEEP : ST_DEAD;
 }
 

@@ -150,7 +150,7 @@ int b200_stage(b200_engine_t *e, const b200_batch_t *b, const b200_stage_conf_t 
             for (int64_t i = b->file_start[f]; i < b->file_start[f + 1]; ++i) {
                 if (e->state[(size_t)i] != ST_KEEP) continue;
                 const int32_t pos = e->desc[(size_t)i].rpos, end = pos + e->rlen[(size_t)i];
-                if (have) {
+                if (have && !(b->rbits && (b->rbits[i] & B200_RB_MAXDEPTH_SEEN))) {   // verdicts of earlier windows stand
                     while (!ends.empty() && ends.top() < pp) ends.pop();
                     if (pos == pp && (int64_t)ends.size() + 1 > (int64_t)cf->max_depth) { e->state[(size_t)i] = ST_MAXDROP; changed = true; continue; }
                 }

@@ -163,10 +163,7 @@ def run_cases(tool, oracle, d, cases, env=None):
 @pytest.mark.parametrize('env', [{}, {'B200_WINDOW_COLS': '4099'}, {'EMUL_GENERAL': '1'}], ids=['default', 'win4099', 'general'])
 def test_emulation_vs_oracle_long_reads(env, long_dir, emul_dir, oracle_bin):
     d, _ = long_dir
-    cases = LONG_CASES
-    if 'B200_WINDOW_COLS' in env:   # the -d buffer occupancy is not carried across a column window's edge (cli.cpp, window_cols)
-        cases = [c for c in cases if ' -d ' not in f' {c[1]} ']
-    bad = run_cases(os.path.join(emul_dir, 'b200samtools_emul'), oracle_bin, d, cases, env)
+    bad = run_cases(os.path.join(emul_dir, 'b200samtools_emul'), oracle_bin, d, LONG_CASES, env)
     assert not bad, bad[:3]
 
 
