@@ -29,7 +29,6 @@
 #include <string>
 #include <vector>
 #include <algorithm>
-#include <queue>
 
 #include "../../include/b200_pileup.h"
 #include "plp_core.h"
@@ -709,9 +708,7 @@ static int max_buffered_reads(b200_engine *e, int *out)
     return 0;
 }
 
-// max-depth rule of bam_plp_push, evaluated on the host only when a column could
-// hold more than maxcnt reads (sequential by nature; see DESIGN.md).  Reads whose verdict an earlier window made
-// (B200_RB_MAXDEPTH_SEEN) are not judged again: the kept ones only fill the buffer, the dropped ones are ST_MAXDROP already.
+// max-depth rule of bam_plp_push (plp_stage.h apply_max_depth) on the host, over copies of the per-read state
 static int apply_maxcnt_host(b200_engine *e, int64_t n, int maxcnt)
 {
     std::vector<ReadDesc> hd((size_t)n);
@@ -720,21 +717,8 @@ static int apply_maxcnt_host(b200_engine *e, int64_t n, int maxcnt)
     CK(cudaMemcpyAsync(st.data(), e->state, (size_t)n, cudaMemcpyDeviceToHost, e->stream));
     if (e->has_rbits) { rb.resize((size_t)n); CK(cudaMemcpyAsync(rb.data(), e->rbits, (size_t)n, cudaMemcpyDeviceToHost, e->stream)); }
     CK(cudaStreamSynchronize(e->stream));
-    bool changed = false;
-    for (int f = 0; f < e->n_files; ++f) {
-        std::priority_queue<int32_t, std::vector<int32_t>, std::greater<int32_t>> ends;  // accepted reads still buffered
-        bool have_prev = false; int32_t p_prev = 0;
-        for (int64_t i = e->h_file_start[f]; i < e->h_file_start[f + 1]; ++i) {
-            if (st[i] != ST_KEEP) continue;
-            const int32_t pos = hd[i].rpos, end = hd[i].rpos + e->h_rlen_tmp[i];
-            if (have_prev && !(e->has_rbits && (rb[i] & B200_RB_MAXDEPTH_SEEN))) {
-                while (!ends.empty() && ends.top() < p_prev) ends.pop();   // buffered = accepted reads with end >= previous accepted start
-                if (pos == p_prev && (int64_t)ends.size() + 1 > (int64_t)maxcnt) { st[i] = ST_MAXDROP; changed = true; continue; }
-            }
-            ends.push(end);
-            have_prev = true; p_prev = pos;
-        }
-    }
+    const bool changed = apply_max_depth(hd.data(), e->h_rlen_tmp.data(), e->has_rbits ? rb.data() : nullptr, st.data(),
+                                         e->h_file_start.data(), e->n_files, maxcnt);
     if (changed) CK(cudaMemcpyAsync(e->state, st.data(), (size_t)n, cudaMemcpyHostToDevice, e->stream));
     e->maxdrop_applied = changed;
     return 0;
@@ -749,11 +733,8 @@ __global__ void k_apply_maxdrop(const uint8_t *state, ReadDesc *desc, int32_t *e
 
 static int stage_device(b200_engine *e, b200_stage_stats_t *stats);
 
-// Some record starts before its predecessor (rare path).  htslib's bam_plp_push rejects a PUSHED read that starts before
-// the previous pushed read of the same file ("The input is not sorted", error return); reads dropped by the filters never
-// reach the push.  The column kernels binary-search the descriptors by start, so unsorted input must not get through:
-// exact check over the kept reads of each file on the host.  depth (bam2depth.c:329-333) tolerates some disorder; here any
-// disorder among its kept reads is refused ("Data is not position sorted") rather than risking silently wrong counts.
+// Some record starts before its predecessor (rare path): the exact sortedness check (plp_stage.h unsorted_error) on the
+// host, over copies of the per-read state
 static int check_sorted_host(b200_engine *e, int64_t n)
 {
     std::vector<ReadDesc> hd((size_t)n);
@@ -761,16 +742,9 @@ static int check_sorted_host(b200_engine *e, int64_t n)
     CK(cudaMemcpyAsync(hd.data(), e->desc, (size_t)n * sizeof(ReadDesc), cudaMemcpyDeviceToHost, e->stream));
     CK(cudaMemcpyAsync(st.data(), e->state, (size_t)n, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
-    for (int f = 0; f < e->n_files; ++f) {
-        bool have = false; int32_t last = 0;
-        for (int64_t i = e->h_file_start[f]; i < e->h_file_start[f + 1]; ++i) {
-            if (st[i] != ST_KEEP) continue;
-            if (have && hd[i].rpos < last) {
-                snprintf(e->err, sizeof e->err, "%s", e->sconf.mode == B200_MODE_DEPTH ? "Data is not position sorted" : "The input is not sorted (reads out of order)");
-                return -3;
-            }
-            have = true; last = hd[i].rpos;
-        }
+    if (const char *msg = unsorted_error(e->sconf, hd.data(), st.data(), e->h_file_start.data(), e->n_files)) {
+        snprintf(e->err, sizeof e->err, "%s", msg);
+        return -3;
     }
     return 0;
 }
@@ -817,13 +791,7 @@ extern "C" int b200_stage(b200_engine_t *e, const b200_batch_t *b, const b200_st
     if (cf->mode == B200_MODE_DEPTH && cf->d_remove_overlaps && b->depth_clip && n > 0) {
         // clip coordinates replayed by the caller (one name hash per file, across reference sequences)
         e->h_clip_tmp.resize((size_t)n);
-        for (int64_t i = 0; i < n; ++i) {
-            const int64_t cabs = b->depth_clip[i];
-            int64_t rel = cabs ? cabs - e->win_base : (int64_t)INT32_MIN;
-            if (rel > INT32_MAX) rel = INT32_MAX;
-            if (rel < INT32_MIN) rel = INT32_MIN;
-            e->h_clip_tmp[(size_t)i] = (int32_t)rel;
-        }
+        for (int64_t i = 0; i < n; ++i) e->h_clip_tmp[(size_t)i] = window_clip(b->depth_clip[i], e->win_base);
         H2D(clip, e->h_clip_tmp.data(), n);
         e->has_host_clip = true;
     }
@@ -885,15 +853,10 @@ static int stage_device(b200_engine *e, b200_stage_stats_t *stats)
     e->sum_rlen = ha.sum_rlen; e->sum_indel_text = ha.sum_indel_text; e->sum_rlen_gen = ha.sum_rlen_gen;
     // ---- column domain
     {
-        int64_t wend = cf->end - e->win_base;                       // exclusive, relative
-        int64_t cov = e->max_rend > 0 ? e->max_rend : 0;
-        if (cov > wend) cov = wend;
-        int64_t allc = (cf->end < e->tid_len ? cf->end : e->tid_len) - e->win_base;
-        if (allc < 0) allc = 0;
-        e->ncols_cov = cov; e->ncols_all = allc;
-        int64_t nc = cov > allc ? cov : allc;
-        if (nc >= (1LL << 31) - 4096) { snprintf(e->err, sizeof e->err, "window too wide (%lld columns)", (long long)nc); return -1; }
-        e->ncols_max = (int32_t)nc;
+        const ColDomain d = column_domain(*cf, e->win_base, e->max_rend, e->tid_len);
+        e->ncols_cov = d.cov; e->ncols_all = d.all;
+        if (d.max() >= (1LL << 31) - 4096) { snprintf(e->err, sizeof e->err, "window too wide (%lld columns)", (long long)d.max()); return -1; }
+        e->ncols_max = (int32_t)d.max();
     }
     e->n_groups = (e->ncols_max + 31) / 32 + 1;
     ENSURE(glo, (size_t)e->n_groups * e->n_files + 1); ENSURE(ghi, (size_t)e->n_groups * e->n_files + 1);

@@ -19,6 +19,7 @@
 #include <math.h>
 #include <zlib.h>
 #include <cctype>
+#include <cstdarg>
 #include <climits>
 #include <cstdio>
 #include <cstdlib>
@@ -99,7 +100,7 @@ struct Engine {
         return true;
     }
 };
-// Devices for the extra window workers of a driver: B200_DEVICES="0,1,2,3" (one handle each), times B200_HANDLES handles per
+// Devices for the window workers of a driver: B200_DEVICES="0,1,2,3" (one handle each), times B200_HANDLES handles per
 // device (default 1).  The column windows of a reference sequence are independent (each stages its own halo), so they are
 // handed round-robin to the workers -- region sharding across GPUs (SURVEY 8e) below the Python layer, and, with several
 // handles on one device, H2D / kernels / D2H of consecutive windows overlapping.  Unset: one handle on B200_DEVICE.
@@ -116,32 +117,58 @@ std::vector<int> worker_devices()
     for (int k = 0; k < per; ++k) for (int dev : d) out.push_back(dev);
     return out;
 }
-void write_all(FILE *fp, const std::vector<char> &buf, size_t n) { if (n) fwrite(buf.data(), 1, n, fp); }
-
-// One extra window worker of a driver: its own engine handle, packer, record cursors and output buffer.
-struct WinWorker { Engine eng; PackedBatch pb; std::vector<char> out; std::vector<size_t> sel, cursor; size_t need = 0; int rc = 0; std::string err; };
-bool make_workers(std::vector<std::unique_ptr<WinWorker>> &workers, int n_files)
+// One engine handle of a driver: its packer, record cursors (one per file) and the output of the window it last ran.
+struct WinWorker {
+    Engine eng; PackedBatch pb; std::vector<char> out; std::vector<size_t> sel, cursor; size_t need = 0; int rc = 0; std::string err;
+    void rewind() { std::fill(cursor.begin(), cursor.end(), 0); }
+    int fail(const char *tool) { rc = -1; err = std::string("samtools ") + tool + ": " + b200_last_error(eng.e); return -1; }
+};
+using Workers = std::vector<std::unique_ptr<WinWorker>>;
+// The handles of a driver, never none: one per entry of worker_devices() where that lists several and the driver can use
+// them (`several`), else one on B200_DEVICE.
+bool make_workers(Workers &workers, int n_files, bool several)
 {
-    const std::vector<int> wd = worker_devices();
-    if (wd.size() < 2) return true;
+    std::vector<int> wd = several ? worker_devices() : std::vector<int>();
+    if (wd.size() < 2) wd.assign(1, -1);
     for (int dev : wd) { workers.emplace_back(new WinWorker()); if (!workers.back()->eng.init(dev)) return false; workers.back()->cursor.assign((size_t)n_files, 0); }
     return true;
 }
-// Rounds of one window per worker: job(worker, wb, we) packs, stages and formats its window concurrently with the others
-// (setting rc / err / need), then the texts are written in window order.
-template <class Job>
-int run_window_rounds(std::vector<std::unique_ptr<WinWorker>> &workers, const std::vector<std::pair<int64_t, int64_t>> &wins, FILE *fp, const char *tool, Job job)
+// printf onto the end of a worker's output
+__attribute__((format(printf, 2, 3))) void appendf(WinWorker &w, const char *fmt, ...)
 {
-    for (auto &w : workers) std::fill(w->cursor.begin(), w->cursor.end(), 0);
-    const size_t K = workers.size();
-    for (size_t base = 0; base < wins.size(); base += K) {
-        const size_t m = std::min(K, wins.size() - base);
-        std::vector<std::thread> th;
-        for (size_t t = 0; t < m; ++t) th.emplace_back([&, t]() { WinWorker &w = *workers[t]; w.rc = 0; w.need = 0; job(w, wins[base + t].first, wins[base + t].second); });
-        for (auto &t : th) t.join();
+    for (;;) {
+        va_list ap;
+        va_start(ap, fmt);
+        const int k = vsnprintf(w.out.data() + w.need, w.out.size() - w.need, fmt, ap);
+        va_end(ap);
+        if (k < 0) return;
+        if (w.need + (size_t)k < w.out.size()) { w.need += (size_t)k; return; }
+        w.out.resize(std::max(2 * w.out.size(), w.need + (size_t)k + 1));
+    }
+}
+
+using Windows = std::vector<std::pair<int64_t, int64_t>>;
+// Rounds of one window per worker over the first k workers: job(worker, wb, we) stages its window concurrently with the
+// others (a round of one window runs on the calling thread) and leaves its text in out[0, need) (or sets rc / err); then
+// the texts are written in window order.
+template <class Job>
+int run_window_rounds(Workers &workers, const Windows &wins, size_t k, FILE *fp, Job job)
+{
+    for (auto &w : workers) w->rewind();
+    k = std::min(k, workers.size());
+    for (size_t base = 0; base < wins.size(); base += k) {
+        const size_t m = std::min(k, wins.size() - base);
+        auto run = [&](size_t t) { WinWorker &w = *workers[t]; w.rc = 0; w.need = 0; job(w, wins[base + t].first, wins[base + t].second); };
+        if (m == 1) run(0);
+        else {
+            std::vector<std::thread> th;
+            for (size_t t = 0; t < m; ++t) th.emplace_back(run, t);
+            for (auto &t : th) t.join();
+        }
         for (size_t t = 0; t < m; ++t) {
-            if (workers[t]->rc != 0) { fprintf(stderr, "samtools %s: %s\n", tool, workers[t]->err.c_str()); return -1; }
-            write_all(fp, workers[t]->out, workers[t]->need);
+            const WinWorker &w = *workers[t];
+            if (w.rc != 0) { fprintf(stderr, "%s\n", w.err.c_str()); return -1; }
+            if (w.need) fwrite(w.out.data(), 1, w.need, fp);
         }
     }
     return 0;
@@ -227,6 +254,42 @@ bool records_extent(const std::vector<FileData> &fd, int tid, int64_t &first, in
         for (const Record &r : f.by_tid[(size_t)tid]) { any = true; if (r.pos < first) first = r.pos; const int64_t e = r.endpos(); if (e > last) last = e; }
     }
     return any;
+}
+// Columns [lo,hi) whose rows mpileup / depth print for contig tid: the region [rb,re), cut down to the span of the records
+// unless empty rows are wanted (`all`), and in that case extended to records running past the contig's end.  Without
+// reads, the region within the contig.  False when the contig's records leave no column to visit.
+bool column_range(const std::vector<FileData> &fd, int tid, int64_t tid_len, int64_t rb, int64_t re, bool all, bool with_reads,
+                  int64_t &lo, int64_t &hi)
+{
+    lo = rb; hi = std::min(re, tid_len);
+    if (!with_reads) return true;
+    int64_t first = 0, last = 0;
+    if (!records_extent(fd, tid, first, last)) return false;
+    if (!all) { lo = std::max(rb, first); hi = std::min(re, last); } else hi = std::max(hi, std::min(re, last));
+    return lo < hi;
+}
+// [lo,hi) cut into windows of window_cols() columns; an empty range is still one (empty) window
+Windows column_windows(int64_t lo, int64_t hi)
+{
+    Windows wins;
+    for (int64_t wb = lo; wb < hi || wb == lo; wb += window_cols()) wins.emplace_back(wb, std::max(std::min(wb + window_cols(), hi), wb));
+    return wins;
+}
+// Stages window [wb,we) of contig tid on worker w: add(i) packs into w.pb the records file i contributes (w.cursor[i] and
+// w.sel are its to use), and `md`, if given, then takes the engine's max-depth verdicts.  A coverage window without records
+// has nothing to count and is not staged (returns 1).  Returns -1 with w.err set on an error.
+template <class Add>
+int stage_window(WinWorker &w, const Header &h, int tid, const std::string *ref, const b200_stage_conf_t &sc, int64_t wb, int64_t we,
+                 MaxDepthCarry *md, const char *tool, b200_stage_stats_t &st, Add add)
+{
+    w.pb.clear();
+    for (int i = 0; i < (int)w.cursor.size(); ++i) { w.pb.begin_file(); add(i); }
+    w.pb.finish();
+    if (sc.mode == B200_MODE_COVERAGE && w.pb.pos.empty()) return 1;
+    b200_batch_t batch = w.pb.view(tid, h.lens[(size_t)tid], h.names[(size_t)tid], ref);
+    b200_stage_conf_t wsc = sc; wsc.beg = wb; wsc.end = we;
+    if (b200_stage(w.eng.e, &batch, &wsc, &st) != 0 || (md && md->collect(w.eng.e) != 0)) return w.fail(tool);
+    return 0;
 }
 
 // ----------------------------------------------------------------------------- mpileup
@@ -319,34 +382,29 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn)
     if (!max_depth) { max_depth = INT_MAX; fprintf(stderr, "[mpileup] Max depth set to maximum value (%d)\n", INT_MAX); }
     else if ((long long)max_depth * nfn > 1 << 20) fprintf(stderr, "[mpileup] Combined max depth is above 1M. Potential memory hog!\n");
 
-    Engine eng;
-    if (!eng.init()) return 1;
+    // window workers (worker_devices()): the text path without host columns can be spread over several handles
+    Workers workers;
+    if (!make_workers(workers, nfn, !o.gl && o.xcols.empty())) return 1;
     b200_stage_conf_t sc; memset(&sc, 0, sizeof sc);
     sc.mode = B200_MODE_MPILEUP; sc.rflag_require = o.rf; sc.rflag_filter = o.ff; sc.min_mq = o.min_mq; sc.no_orphan = o.no_orphan;
     sc.illumina13 = o.illumina13; sc.baq = o.realn ? (o.redo_baq ? 2 : 1) : 0; sc.capq_thres = o.capQ; sc.overlaps = o.overlaps;
-    sc.max_depth = max_depth; sc.beg = o.reg ? beg0 : 0; sc.end = o.reg ? end0 : POS_MAX;
+    sc.max_depth = max_depth;
     b200_mpileup_conf_t mc; memset(&mc, 0, sizeof mc);
     mc.min_baseQ = o.min_baseQ; mc.all = o.all; mc.rev_del = o.rev_del; mc.no_ins = o.no_ins; mc.no_del = o.no_del; mc.no_ends = o.no_ends;
     mc.out_mapq = o.out_mapq; mc.out_qpos = o.out_qpos; mc.out_qpos5 = o.out_qpos5;
 
-    PackedBatch pb;
-    std::vector<char> out;
     std::vector<int64_t> bb, be;
     const int nref = h.n_ref();
-    // extra window workers (worker_devices()): the text path without host columns can be spread over several handles
-    std::vector<std::unique_ptr<WinWorker>> workers;
-    if (!o.gl && o.xcols.empty() && !make_workers(workers, nfn)) return 1;
-    std::vector<size_t> sel; std::vector<size_t> cursor((size_t)nfn);
     std::vector<std::vector<uint8_t>> hbits((size_t)nfn);   // host bits of the contig's records, decided ONCE (the BQ:Z path edits the record)
     std::vector<const Record *> staged;                     // records of the staged window, batch order (host columns)
     std::vector<uint32_t> x_off; std::string x_dat; std::vector<uint8_t> x_mapq;
     // per-read strings of the host columns (--output-QNAME / --output-extra, bam_plcmd.c:727-855) for the staged window
-    auto render_host_columns = [&]() -> int {
+    auto render_host_columns = [&](WinWorker &w) -> int {
         const size_t nr = staged.size(), nx = o.xcols.size();
         x_off.assign(nx * (nr + 1), 0); x_dat.clear();
         bool need_mapq = false;
         for (const std::string &cname : o.xcols) if (cname == "MAPQ") need_mapq = true;
-        if (need_mapq && nr) { x_mapq.resize(nr); if (b200_fetch_mapq_keep(eng.e, x_mapq.data(), nullptr, nr) != 0) return -1; }   // after -C
+        if (need_mapq && nr) { x_mapq.resize(nr); if (b200_fetch_mapq_keep(w.eng.e, x_mapq.data(), nullptr, nr) != 0) return -1; }   // after -C
         char tmp[64];
         for (size_t k = 0; k < nx; ++k) {
             const std::string &cname = o.xcols[k];
@@ -388,121 +446,77 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn)
         return 0;
     };
     MaxDepthCarry md;
-    // one window [wb,we) of contig tid (cont: it continues an earlier window): stage the overlapping records, return the
-    // stage statistics
-    auto stage_window = [&](int tid, bool with_reads, int64_t wb, int64_t we, bool cont, const std::string *ref, b200_stage_stats_t &st) -> int {
-        const std::string &name = h.names[(size_t)tid];
-        pb.clear(); staged.clear();
-        for (int i = 0; i < nfn; ++i) {
-            pb.begin_file();
-            if (with_reads && tid < (int)fd[(size_t)i].by_tid.size()) {
-                std::vector<Record> &v = fd[(size_t)i].by_tid[(size_t)tid];
-                window_records(v, cursor[(size_t)i], wb, we, sel, cont);
-                for (size_t j : sel) { pb.add(v[j], (uint8_t)(hbits[(size_t)i][j] | md.add(i, j)), o.overlaps); if (!o.xcols.empty()) staged.push_back(&v[j]); }
-            }
-        }
-        pb.finish();
-        b200_batch_t batch = pb.view(tid, h.lens[(size_t)tid], name, ref);
-        sc.beg = wb; sc.end = we;
-        if (b200_stage(eng.e, &batch, &sc, &st) != 0 || md.collect(eng.e) != 0) { fprintf(stderr, "samtools mpileup: %s\n", b200_last_error(eng.e)); return -1; }
-        return 0;
-    };
     auto process_tid = [&](int tid, bool with_reads) -> int {
         // returns 1 when rows were requested and produced, 0 when the contig has no pileup column, <0 on error
         const std::string &name = h.names[(size_t)tid];
         const std::string *ref = nullptr;
         if (o.fa) { int fi = o.fa->find(name); if (fi >= 0) ref = &o.fa->seqs[(size_t)fi]; }
         if (o.bed) { o.bed->merged(name, bb, be); mc.bed_beg = bb.data(); mc.bed_end = be.data(); mc.n_bed = (int)bb.size(); mc.bed_active = 1; }
-        // columns to visit: the region, cut down to the span of the records unless empty rows are wanted (-a)
-        const int64_t rb = o.reg ? beg0 : 0, re = o.reg ? end0 : POS_MAX, tid_len = h.lens[(size_t)tid];
-        int64_t first = 0, last = 0;
-        const bool have = with_reads && records_extent(fd, tid, first, last);
-        int64_t lo_col = rb, hi_col = std::min(re, tid_len);
-        if (have) { if (!o.all) { lo_col = std::max(rb, first); hi_col = std::min(re, last); } else hi_col = std::max(hi_col, std::min(re, last)); }
-        else if (with_reads) return 0;
+        int64_t lo = 0, hi = 0;
+        if (!column_range(fd, tid, h.lens[(size_t)tid], beg0, end0, o.all, with_reads, lo, hi)) return 0;
         for (int i = 0; i < nfn; ++i) {
             hbits[(size_t)i].clear();
             if (with_reads && tid < (int)fd[(size_t)i].by_tid.size())
                 for (Record &r : fd[(size_t)i].by_tid[(size_t)tid]) hbits[(size_t)i].push_back(mp_host_bits(o, h, r, ref != nullptr));
         }
-        const int64_t W = window_cols();
+        const Windows wins = column_windows(lo, hi);
+        // a window that continues an earlier one also takes the records ending at its start (the -d rule's closed intervals)
+        auto stage = [&](WinWorker &w, int64_t wb, int64_t we, b200_stage_stats_t &st) {
+            if (!o.xcols.empty()) staged.clear();
+            return stage_window(w, h, tid, ref, sc, wb, we, &md, "mpileup", st, [&](int i) {
+                if (!with_reads || tid >= (int)fd[(size_t)i].by_tid.size()) return;
+                std::vector<Record> &v = fd[(size_t)i].by_tid[(size_t)tid];
+                window_records(v, w.cursor[(size_t)i], wb, we, w.sel, wb > lo);
+                for (size_t j : w.sel) { w.pb.add(v[j], (uint8_t)(hbits[(size_t)i][j] | md.add(i, j)), o.overlaps); if (!o.xcols.empty()) staged.push_back(&v[j]); }
+            });
+        };
         // the first window with a pileup column decides whether the contig is reported at all (its empty -a rows before that
         // column included), so find it before anything is written
-        int64_t first_hit = -1;
         md.reset(fd, tid, false);
         if (with_reads) {
-            std::fill(cursor.begin(), cursor.end(), 0);
-            for (int64_t wb = lo_col; wb < hi_col; wb += W) {
+            WinWorker &w = *workers[0];
+            w.rewind();
+            bool hit = false;
+            for (size_t k = 0; k < wins.size() && !hit; ++k) {
                 b200_stage_stats_t st;
-                if (stage_window(tid, true, wb, std::min(wb + W, hi_col), wb > lo_col, ref, st) != 0) return -1;
-                if (st.n_kept_in_window > 0) { first_hit = wb; break; }
+                if (stage(w, wins[k].first, wins[k].second, st) != 0) { fprintf(stderr, "%s\n", w.err.c_str()); return -1; }
+                hit = st.n_kept_in_window > 0;
             }
-            if (first_hit < 0) return 0;
+            if (!hit) return 0;
         }
-        // a contig split into several windows where the max-depth rule may fire runs them in order, each handing its
-        // verdicts to the next; elsewhere the windows are independent
-        const bool carry = with_reads && hi_col - lo_col > W && max_stacked_records(fd, tid) > (int64_t)max_depth;
-        if (with_reads && !workers.empty() && !carry) {
-            std::vector<std::pair<int64_t, int64_t>> wins;
-            for (int64_t wb = lo_col; wb < hi_col; wb += W) wins.emplace_back(wb, std::min(wb + W, hi_col));
-            const int rc = run_window_rounds(workers, wins, fp, "mpileup", [&](WinWorker &w, int64_t wb, int64_t we) {
-                w.pb.clear();
-                for (int i = 0; i < nfn; ++i) {
-                    w.pb.begin_file();
-                    if (tid < (int)fd[(size_t)i].by_tid.size()) {
-                        std::vector<Record> &v = fd[(size_t)i].by_tid[(size_t)tid];
-                        window_records(v, w.cursor[(size_t)i], wb, we, w.sel, wb > lo_col);
-                        for (size_t j : w.sel) w.pb.add(v[j], hbits[(size_t)i][j], o.overlaps);
-                    }
-                }
-                w.pb.finish();
-                b200_batch_t batch = w.pb.view(tid, h.lens[(size_t)tid], name, ref);
-                b200_stage_conf_t wsc = sc; wsc.beg = wb; wsc.end = we;
-                b200_stage_stats_t st;
-                if (b200_stage(w.eng.e, &batch, &wsc, &st) != 0) { w.rc = -1; w.err = b200_last_error(w.eng.e); return; }
-                if (!o.all && st.n_kept_in_window == 0) return;
-                const size_t bound = (size_t)b200_mpileup_text_bound(w.eng.e, &mc);
-                if (w.out.size() < bound + 64) w.out.resize(bound + 64);
-                if (b200_mpileup_text(w.eng.e, &mc, w.out.data(), w.out.size(), &w.need) != 0) { w.rc = -1; w.err = b200_last_error(w.eng.e); }
-            });
-            if (rc != 0) return -1;
-            return 1;
-        }
-        std::fill(cursor.begin(), cursor.end(), 0);
+        // a contig split into several windows where the max-depth rule may fire runs them in order on worker 0, each handing
+        // its verdicts to the next; so do the empty rows of a contig without reads (GL and host columns have one worker).
+        // Elsewhere the windows are independent.
+        const bool carry = with_reads && wins.size() > 1 && max_stacked_records(fd, tid) > (int64_t)max_depth;
         md.reset(fd, tid, carry);
-        for (int64_t wb = lo_col; wb < hi_col || (!with_reads && wb == lo_col); wb += W) {
-            const int64_t we = std::max(std::min(wb + W, hi_col), wb);
+        const int rc = run_window_rounds(workers, wins, carry || !with_reads ? 1 : workers.size(), fp, [&](WinWorker &w, int64_t wb, int64_t we) {
             b200_stage_stats_t st;
-            if (stage_window(tid, with_reads, wb, we, wb > lo_col, ref, st) != 0) return -1;
-            if (with_reads && !o.all && st.n_kept_in_window == 0) continue;
+            if (stage(w, wb, we, st) != 0) return;
+            if (with_reads && !o.all && st.n_kept_in_window == 0) return;
             if (o.gl) {
                 int64_t ncols = 0; const size_t cap = (size_t)st.n_cols + 16;
                 std::vector<int64_t> cpos(cap); std::vector<int32_t> nb(cap * (size_t)nfn); std::vector<float> qs(cap * (size_t)nfn * 4), p25(cap * (size_t)nfn * 25);
-                if (b200_glf(eng.e, o.min_baseQ, &ncols, cpos.data(), nb.data(), qs.data(), p25.data(), cap) != 0) { fprintf(stderr, "samtools gl: %s\n", b200_last_error(eng.e)); return -1; }
+                if (b200_glf(w.eng.e, o.min_baseQ, &ncols, cpos.data(), nb.data(), qs.data(), p25.data(), cap) != 0) { w.fail("gl"); return; }
                 for (int64_t k = 0; k < ncols; ++k) {
                     const int64_t p = cpos[(size_t)k];
                     if (o.bed && !o.bed->overlap(name, p, p + 1)) continue;
-                    fprintf(fp, "%s\t%lld\t%c", name.c_str(), (long long)p + 1, (ref && p < (int64_t)ref->size()) ? (*ref)[(size_t)p] : 'N');
+                    appendf(w, "%s\t%lld\t%c", name.c_str(), (long long)p + 1, (ref && p < (int64_t)ref->size()) ? (*ref)[(size_t)p] : 'N');
                     for (int f = 0; f < nfn; ++f) {
                         const size_t d = (size_t)k * (size_t)nfn + (size_t)f;
-                        fprintf(fp, "\t%d", nb[d] < 0 ? 0 : nb[d]);
-                        for (int j = 0; j < 4; ++j) fprintf(fp, "\t%.9g", qs[d * 4 + (size_t)j]);
-                        for (int j = 0; j < 25; ++j) fprintf(fp, "\t%.9g", p25[d * 25 + (size_t)j]);
+                        appendf(w, "\t%d", nb[d] < 0 ? 0 : nb[d]);
+                        for (int j = 0; j < 4; ++j) appendf(w, "\t%.9g", qs[d * 4 + (size_t)j]);
+                        for (int j = 0; j < 25; ++j) appendf(w, "\t%.9g", p25[d * 25 + (size_t)j]);
                     }
-                    fputc('\n', fp);
+                    appendf(w, "\n");
                 }
-                continue;
+                return;
             }
-            if (!o.xcols.empty() && render_host_columns() != 0) { fprintf(stderr, "samtools mpileup: %s\n", b200_last_error(eng.e)); return -1; }
-            const size_t bound = (size_t)b200_mpileup_text_bound(eng.e, &mc);
-            if (out.size() < bound + 64) out.resize(bound + 64);
-            size_t need = 0;
-            int rc = b200_mpileup_text(eng.e, &mc, out.data(), out.size(), &need);      // format and fetch in one call
-            if (rc != 0) { fprintf(stderr, "samtools mpileup: %s\n", b200_last_error(eng.e)); return -1; }
-            write_all(fp, out, need);
-            if (!with_reads) break;
-        }
-        return 1;
+            if (!o.xcols.empty() && render_host_columns(w) != 0) { w.fail("mpileup"); return; }
+            const size_t bound = (size_t)b200_mpileup_text_bound(w.eng.e, &mc);
+            if (w.out.size() < bound + 64) w.out.resize(bound + 64);
+            if (b200_mpileup_text(w.eng.e, &mc, w.out.data(), w.out.size(), &w.need) != 0) w.fail("mpileup");   // format and fetch in one call
+        });
+        return rc != 0 ? -1 : 1;
     };
 
     // contigs that yield at least one pileup column inside the region, in order (bam_plcmd.c:607-609)
@@ -684,14 +698,14 @@ int main_depth(int argc, char **argv)
     FILE *fp = out_fn ? fopen(out_fn, "w") : stdout;
     if (!fp) { fprintf(stderr, "samtools depth: Cannot open \"%s\" for writing.\n", out_fn); return 1; }
     if (header) { fprintf(fp, "#CHROM\tPOS"); for (auto &f : fn) fprintf(fp, "\t%s", f.c_str()); fputc('\n', fp); }
-    Engine eng;
-    if (!eng.init()) return 1;
+    Workers workers;      // window workers (worker_devices())
+    if (!make_workers(workers, nfn, true)) return 1;
     b200_stage_conf_t sc; memset(&sc, 0, sizeof sc);
     sc.mode = B200_MODE_DEPTH; sc.d_flag_excl = flag; sc.d_flag_incl = incl; sc.d_flag_require = require; sc.d_min_mapq = min_mqual;
-    sc.d_min_len = min_len; sc.d_remove_overlaps = remove_overlaps; sc.beg = reg ? beg0 : 0; sc.end = reg ? end0 : POS_MAX;
+    sc.d_min_len = min_len; sc.d_remove_overlaps = remove_overlaps;
     b200_depth_conf_t dc; memset(&dc, 0, sizeof dc);
     dc.min_qual = min_qual; dc.count_del = !skip_del; dc.all = all_pos;
-    PackedBatch pb; std::vector<char> out; std::vector<int64_t> bb, be;
+    std::vector<int64_t> bb, be;
     // depth -s: the reference keeps one qname -> end-position hash PER FILE for the whole run (bam2depth.c:598-623),
     // i.e. across reference sequences, and only records that pass the read filters take part.  It is replayed here
     // in file order (name hashing is host work anyway) and handed to the engine as one clip coordinate per record.
@@ -726,89 +740,43 @@ int main_depth(int argc, char **argv)
             cv.push_back(clip);
         }
     };
-    std::vector<size_t> sel; std::vector<size_t> cursor((size_t)nfn);
-    std::vector<std::unique_ptr<WinWorker>> workers;      // extra window workers (worker_devices())
-    if (!make_workers(workers, nfn)) return 1;
-    auto stage_window = [&](int tid, bool with_reads, int64_t wb, int64_t we, b200_stage_stats_t &st) -> int {
-        pb.clear();
-        for (int i = 0; i < nfn; ++i) {
-            pb.begin_file();
-            if (with_reads && tid < (int)fd[(size_t)i].by_tid.size()) {
-                std::vector<Record> &v = fd[(size_t)i].by_tid[(size_t)tid];
-                window_records(v, cursor[(size_t)i], wb, we, sel);
-                for (size_t j : sel) {
-                    pb.add(v[j], 0, false);
-                    if (remove_overlaps) pb.depth_clip.push_back(clips[(size_t)i][(size_t)tid][j]);
-                }
-            }
-        }
-        pb.finish();
-        b200_batch_t batch = pb.view(tid, h.lens[(size_t)tid], h.names[(size_t)tid], nullptr);
-        sc.beg = wb; sc.end = we;
-        if (b200_stage(eng.e, &batch, &sc, &st) != 0) { fprintf(stderr, "samtools depth: %s\n", b200_last_error(eng.e)); return -1; }
-        return 0;
-    };
     auto process_tid = [&](int tid, bool with_reads) -> int {
         const std::string &name = h.names[(size_t)tid];
         if (bed) { bed->merged(name, bb, be); dc.bed_beg = bb.data(); dc.bed_end = be.data(); dc.n_bed = (int)bb.size(); dc.bed_active = 1; }
-        const int64_t rb = reg ? beg0 : 0, re = reg ? end0 : POS_MAX, tid_len = h.lens[(size_t)tid];
-        int64_t first = 0, last = 0;
-        const bool have = with_reads && records_extent(fd, tid, first, last);
-        int64_t lo_col = rb, hi_col = std::min(re, tid_len);
-        if (have) { if (!all_pos) { lo_col = std::max(rb, first); hi_col = std::min(re, last); } else hi_col = std::max(hi_col, std::min(re, last)); }
-        else if (with_reads) return 0;
-        const int64_t W = window_cols();
+        int64_t lo = 0, hi = 0;
+        if (!column_range(fd, tid, h.lens[(size_t)tid], beg0, end0, all_pos, with_reads, lo, hi)) return 0;
+        const Windows wins = column_windows(lo, hi);
+        auto stage = [&](WinWorker &w, int64_t wb, int64_t we, b200_stage_stats_t &st) {
+            return stage_window(w, h, tid, nullptr, sc, wb, we, nullptr, "depth", st, [&](int i) {
+                if (!with_reads || tid >= (int)fd[(size_t)i].by_tid.size()) return;
+                std::vector<Record> &v = fd[(size_t)i].by_tid[(size_t)tid];
+                window_records(v, w.cursor[(size_t)i], wb, we, w.sel);
+                for (size_t j : w.sel) {
+                    w.pb.add(v[j], 0, false);
+                    if (remove_overlaps) w.pb.depth_clip.push_back(clips[(size_t)i][(size_t)tid][j]);
+                }
+            });
+        };
         if (with_reads) {   // a contig no record of which survives the filters is never "seen" (bam2depth.c:255-263): decide before writing
+            WinWorker &w = *workers[0];
+            w.rewind();
             bool seen = false;
-            std::fill(cursor.begin(), cursor.end(), 0);
-            for (int64_t wb = lo_col; wb < hi_col && !seen; wb += W) {
+            for (size_t k = 0; k < wins.size() && !seen; ++k) {
                 b200_stage_stats_t st;
-                if (stage_window(tid, true, wb, std::min(wb + W, hi_col), st) != 0) return -1;
+                if (stage(w, wins[k].first, wins[k].second, st) != 0) { fprintf(stderr, "%s\n", w.err.c_str()); return -1; }
                 seen = st.n_kept > 0;
             }
             if (!seen) return 0;
         }
-        if (with_reads && !workers.empty()) {
-            std::vector<std::pair<int64_t, int64_t>> wins;
-            for (int64_t wb = lo_col; wb < hi_col; wb += W) wins.emplace_back(wb, std::min(wb + W, hi_col));
-            const int rc = run_window_rounds(workers, wins, fp, "depth", [&](WinWorker &w, int64_t wb, int64_t we) {
-                w.pb.clear();
-                for (int i = 0; i < nfn; ++i) {
-                    w.pb.begin_file();
-                    if (tid < (int)fd[(size_t)i].by_tid.size()) {
-                        std::vector<Record> &v = fd[(size_t)i].by_tid[(size_t)tid];
-                        window_records(v, w.cursor[(size_t)i], wb, we, w.sel);
-                        for (size_t j : w.sel) {
-                            w.pb.add(v[j], 0, false);
-                            if (remove_overlaps) w.pb.depth_clip.push_back(clips[(size_t)i][(size_t)tid][j]);
-                        }
-                    }
-                }
-                w.pb.finish();
-                b200_batch_t batch = w.pb.view(tid, h.lens[(size_t)tid], h.names[(size_t)tid], nullptr);
-                b200_stage_conf_t wsc = sc; wsc.beg = wb; wsc.end = we;
-                b200_stage_stats_t st;
-                if (b200_stage(w.eng.e, &batch, &wsc, &st) != 0) { w.rc = -1; w.err = b200_last_error(w.eng.e); return; }
-                const size_t bound = (size_t)b200_depth_text_bound(w.eng.e);
-                if (w.out.size() < bound + 64) w.out.resize(bound + 64);
-                if (b200_depth_text(w.eng.e, &dc, w.out.data(), w.out.size(), &w.need) != 0) { w.rc = -1; w.err = b200_last_error(w.eng.e); }
-            });
-            if (rc != 0) return -1;
-            return 1;
-        }
-        std::fill(cursor.begin(), cursor.end(), 0);
-        for (int64_t wb = lo_col; wb < hi_col || (!with_reads && wb == lo_col); wb += W) {
-            const int64_t we = std::max(std::min(wb + W, hi_col), wb);
+        // the empty rows of a contig without reads run on worker 0 alone
+        const int rc = run_window_rounds(workers, wins, with_reads ? workers.size() : 1, fp, [&](WinWorker &w, int64_t wb, int64_t we) {
             b200_stage_stats_t st;
-            if (stage_window(tid, with_reads, wb, we, st) != 0) return -1;
-            const size_t bound = (size_t)b200_depth_text_bound(eng.e);
-            if (out.size() < bound + 64) out.resize(bound + 64);
-            size_t need = 0;
-            if (b200_depth_text(eng.e, &dc, out.data(), out.size(), &need) != 0) { fprintf(stderr, "samtools depth: %s\n", b200_last_error(eng.e)); return -1; }
-            write_all(fp, out, need);
-            if (!with_reads) break;
-        }
-        return 1;
+            if (stage(w, wb, we, st) != 0) return;
+            const size_t bound = (size_t)b200_depth_text_bound(w.eng.e);
+            if (w.out.size() < bound + 64) w.out.resize(bound + 64);
+            if (b200_depth_text(w.eng.e, &dc, w.out.data(), w.out.size(), &w.need) != 0) w.fail("depth");
+        });
+        return rc != 0 ? -1 : 1;
     };
     const int nref = h.n_ref();
     bool any = false;
@@ -888,8 +856,8 @@ int main_coverage(int argc, char **argv)
     const Header &h = fd[0].rd->header();
     FILE *fp = (out_fn && strcmp(out_fn, "-")) ? fopen(out_fn, "w") : stdout;
     if (!fp) { fprintf(stderr, "samtools coverage: Cannot open \"%s\" for writing.\n", out_fn); return 1; }
-    Engine eng;
-    if (!eng.init()) return 1;
+    Workers workers;
+    if (!make_workers(workers, nfn, false)) return 1;
     const int nref = h.n_ref();
     struct Row { b200_coverage_sums_t s; uint64_t n_sel = 0, sum_mq = 0, n_reads = 0; bool covered = false; int64_t beg = 0, end = 0, bin_width = 1; int n_bins = 0; std::vector<uint32_t> hist; };
     std::vector<Row> rows((size_t)nref);
@@ -897,9 +865,9 @@ int main_coverage(int argc, char **argv)
     sc.mode = B200_MODE_COVERAGE; sc.rflag_filter = fail_flags; sc.rflag_require = required_flags; sc.min_mq = min_mapQ; sc.c_min_len = min_len;
     sc.max_depth = max_depth > 0 ? max_depth : (max_depth == 0 ? INT_MAX : 8000);
     b200_coverage_conf_t cc; cc.min_baseQ = min_baseQ; cc.min_depth = mindepth;
-    PackedBatch pb;
     bool warn = false;
     std::vector<int> order;   // contigs in the order their first column appears
+    MaxDepthCarry md;
     for (int tid = 0; tid < nref; ++tid) {
         Row &rw = rows[(size_t)tid];
         memset(&rw.s, 0, sizeof rw.s);
@@ -919,41 +887,31 @@ int main_coverage(int argc, char **argv)
         // the first / last window also take the records that lie before / beyond the region.
         // A window that continues an earlier one also stages the records ending right at its start (the closed intervals
         // of the -d rule; they cover none of its columns), and where the rule may fire the windows hand their verdicts on.
-        const int64_t W = window_cols();
-        std::vector<size_t> sel, cursor((size_t)nfn, 0);
-        MaxDepthCarry md;
-        md.reset(fd, tid, rw.end - rw.beg > W && max_stacked_records(fd, tid) > (int64_t)sc.max_depth);
-        for (int64_t wb = rw.beg; wb < rw.end || wb == rw.beg; wb += W) {
-            const bool first_w = wb == rw.beg, last_w = wb + W >= rw.end;
-            const int64_t we = last_w ? std::max(rw.end, wb) : wb + W;
-            pb.clear();
-            for (i = 0; i < nfn; ++i) {
-                pb.begin_file();
-                if (tid >= (int)fd[(size_t)i].by_tid.size()) continue;
-                std::vector<Record> &v = fd[(size_t)i].by_tid[(size_t)tid];
-                window_records(v, cursor[(size_t)i], first_w ? INT64_MIN : wb, last_w ? POS_MAX : we, sel, !first_w);
-                for (size_t j : sel) pb.add(v[j], (uint8_t)(((!first_w && v[j].pos < wb) ? B200_RB_HALO : 0) | md.add(i, j)), false);
-            }
-            pb.finish();
-            if (pb.pos.empty()) { md.staged.clear(); if (last_w) break; continue; }
-            b200_batch_t batch = pb.view(tid, h.lens[(size_t)tid], h.names[(size_t)tid], nullptr);
-            sc.beg = wb; sc.end = we;
+        const Windows wins = column_windows(rw.beg, rw.end);
+        md.reset(fd, tid, wins.size() > 1 && max_stacked_records(fd, tid) > (int64_t)sc.max_depth);
+        const int rc = run_window_rounds(workers, wins, 1, fp, [&](WinWorker &w, int64_t wb, int64_t we) {
+            const bool first_w = wb == rw.beg, last_w = we >= rw.end;
             b200_stage_stats_t st;
-            if (b200_stage(eng.e, &batch, &sc, &st) != 0 || md.collect(eng.e) != 0) { fprintf(stderr, "samtools coverage: %s\n", b200_last_error(eng.e)); return 1; }
+            if (stage_window(w, h, tid, nullptr, sc, wb, we, &md, "coverage", st, [&](int i) {
+                    if (tid >= (int)fd[(size_t)i].by_tid.size()) return;
+                    std::vector<Record> &v = fd[(size_t)i].by_tid[(size_t)tid];
+                    window_records(v, w.cursor[(size_t)i], first_w ? INT64_MIN : wb, last_w ? POS_MAX : we, w.sel, !first_w);
+                    for (size_t j : w.sel) w.pb.add(v[j], (uint8_t)(((!first_w && v[j].pos < wb) ? B200_RB_HALO : 0) | md.add(i, j)), false);
+                }) != 0) return;
             rw.n_sel += st.n_selected_reads; rw.sum_mq += st.summed_mapq; rw.n_reads += st.n_reads;
             // a column exists as soon as one kept read has a non-empty reference span (before the region test)
             if (st.n_kept > 0) {
                 b200_coverage_sums_t ws;
-                if (b200_coverage(eng.e, &cc, &ws) != 0) { fprintf(stderr, "samtools coverage: %s\n", b200_last_error(eng.e)); return 1; }
+                if (b200_coverage(w.eng.e, &cc, &ws) != 0) { w.fail("coverage"); return; }
                 rw.s.n_covered_bases += ws.n_covered_bases; rw.s.summed_coverage += ws.summed_coverage; rw.s.summed_baseQ += ws.summed_baseQ;
                 rw.s.quality_bases += ws.quality_bases; rw.s.missing_qual += ws.missing_qual;
                 if (!rw.covered) { rw.covered = true; order.push_back(tid); }   // refined: zero-span-only contigs are vanishingly rare
                 if (ws.missing_qual) warn = true;
                 if (want_hist && rw.n_bins > 0 && rw.bin_width > 0 &&
-                    b200_coverage_hist(eng.e, &cc, rw.beg, rw.bin_width, rw.n_bins, plot_depth ? 1 : 0, rw.hist.data()) != 0) { fprintf(stderr, "samtools coverage: %s\n", b200_last_error(eng.e)); return 1; }
+                    b200_coverage_hist(w.eng.e, &cc, rw.beg, rw.bin_width, rw.n_bins, plot_depth ? 1 : 0, rw.hist.data()) != 0) w.fail("coverage");
             }
-            if (last_w) break;
-        }
+        });
+        if (rc != 0) return 1;
     }
     auto print_row = [&](int tid) {
         const Row &r = rows[(size_t)tid];

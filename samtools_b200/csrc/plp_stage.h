@@ -11,8 +11,11 @@
 //   tweak_overlap htslib sam.c tweak_overlap_quality (doc/samtools-mpileup.1:353-365)
 //   overlap_chain htslib sam.c overlap_push / overlap_remove
 //   depth_clip_chain  olap_hash logic         bam2depth.c:598-623
+//   apply_max_depth   bam_plp_push max-depth rule (htslib sam.c)
 #pragma once
 #include <math.h>
+#include <queue>
+#include <vector>
 #include "../../include/b200_pileup.h"
 #include "plp_core.h"
 
@@ -207,7 +210,7 @@ PLP_HD void stage_build_desc(const RawSoA &r, const b200_stage_conf_t &cf, int64
         }
     }
     desc[i] = d;
-    if (i > 0 && r.pos[i] < r.pos[i - 1]) PLP_ADD64(&acc->n_desc, 1);   // bam_plp_push rejects unsorted input; see check_sorted_host()
+    if (i > 0 && r.pos[i] < r.pos[i - 1]) PLP_ADD64(&acc->n_desc, 1);   // bam_plp_push rejects unsorted input; see unsorted_error()
     // end used for the running max that bounds the per-group read slices: capped at rpos + kReach, because from
     // there on the read is served through the far-reaching lists (k_ovf_*) and must not widen the slices under it
     endv[i] = d.rend > d.rpos ? (d.rend - d.rpos > kReach ? d.rpos + kReach : d.rend) : INT32_MIN;
@@ -434,6 +437,79 @@ PLP_HD void depth_clip_chain(const RawSoA &r, int64_t i, const int64_t *next, co
             have = false;
         }
     }
+}
+
+
+// ---- host rules -----------------------------------------------------------
+// Rules of the read stage that run on the host over the whole staged batch (engine.cu, after copying the per-read state
+// back; the emulation harness directly).  Host-only: the max-depth sweep is sequential by nature.
+
+// Some record starts before its predecessor (rare path).  htslib's bam_plp_push rejects a PUSHED read that starts before
+// the previous pushed read of the same file ("The input is not sorted", error return); reads dropped by the filters never
+// reach the push.  The column kernels binary-search the descriptors by start, so unsorted input must not get through:
+// exact check over the kept reads of each file.  depth (bam2depth.c:329-333) tolerates some disorder; here any disorder
+// among its kept reads is refused ("Data is not position sorted") rather than risking silently wrong counts.
+// Returns the error message, or nullptr when the kept reads are sorted.
+inline const char *unsorted_error(const b200_stage_conf_t &cf, const ReadDesc *desc, const uint8_t *state, const int64_t *file_start, int n_files)
+{
+    for (int f = 0; f < n_files; ++f) {
+        bool have = false; int32_t last = 0;
+        for (int64_t i = file_start[f]; i < file_start[f + 1]; ++i) {
+            if (state[i] != ST_KEEP) continue;
+            if (have && desc[i].rpos < last) return cf.mode == B200_MODE_DEPTH ? "Data is not position sorted" : "The input is not sorted (reads out of order)";
+            have = true; last = desc[i].rpos;
+        }
+    }
+    return nullptr;
+}
+
+// max-depth rule of bam_plp_push, evaluated only when a column could hold more than max_depth reads (see DESIGN.md).
+// Reads whose verdict an earlier window made (B200_RB_MAXDEPTH_SEEN) are not judged again: the kept ones only fill the
+// buffer, the dropped ones are ST_MAXDROP already.  Returns whether a read was dropped here.
+inline bool apply_max_depth(const ReadDesc *desc, const int32_t *rlen, const uint8_t *rbits, uint8_t *state, const int64_t *file_start,
+                            int n_files, int max_depth)
+{
+    bool changed = false;
+    for (int f = 0; f < n_files; ++f) {
+        std::priority_queue<int32_t, std::vector<int32_t>, std::greater<int32_t>> ends;  // accepted reads still buffered
+        bool have_prev = false; int32_t p_prev = 0;
+        for (int64_t i = file_start[f]; i < file_start[f + 1]; ++i) {
+            if (state[i] != ST_KEEP) continue;
+            const int32_t pos = desc[i].rpos, end = desc[i].rpos + rlen[i];
+            if (have_prev && !(rbits && (rbits[i] & B200_RB_MAXDEPTH_SEEN))) {
+                while (!ends.empty() && ends.top() < p_prev) ends.pop();   // buffered = accepted reads with end >= previous accepted start
+                if (pos == p_prev && (int64_t)ends.size() + 1 > (int64_t)max_depth) { state[i] = ST_MAXDROP; changed = true; continue; }
+            }
+            ends.push(end);
+            have_prev = true; p_prev = pos;
+        }
+    }
+    return changed;
+}
+
+// depth -s: a clip coordinate the caller replayed (absolute, 0 = none) relative to the window start, saturated to int32
+inline int32_t window_clip(int64_t clip, int64_t win_base)
+{
+    int64_t rel = clip ? clip - win_base : (int64_t)INT32_MIN;
+    if (rel > INT32_MAX) rel = INT32_MAX;
+    if (rel < INT32_MIN) rel = INT32_MIN;
+    return (int32_t)rel;
+}
+
+// Columns of a staged window, relative to its start: `cov` up to the end of the kept reads (max_rend, 0 without kept
+// reads), `all` up to the contig's end (the -a rows); both cut at the region's end.
+struct ColDomain {
+    int64_t cov, all;
+    int64_t max() const { return cov > all ? cov : all; }
+};
+inline ColDomain column_domain(const b200_stage_conf_t &cf, int64_t win_base, int32_t max_rend, int64_t tid_len)
+{
+    ColDomain d;
+    d.cov = max_rend > 0 ? max_rend : 0;
+    if (d.cov > cf.end - win_base) d.cov = cf.end - win_base;
+    d.all = (cf.end < tid_len ? cf.end : tid_len) - win_base;
+    if (d.all < 0) d.all = 0;
+    return d;
 }
 
 

@@ -16,7 +16,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <queue>
 #include <string>
 #include <vector>
 
@@ -125,52 +124,22 @@ int b200_stage(b200_engine_t *e, const b200_batch_t *b, const b200_stage_conf_t 
     }
     for (int64_t i = 0; i < n; ++i) stage_prep2(r, *cf, i, e->state.data());
     for (int64_t i = 0; i < n; ++i) stage_build_desc(r, *cf, i, e->state.data(), e->rlen.data(), e->desc.data(), e->endv.data(), &e->acc, e->win_base, e->cig_x.data(), e->cig_y.data());
-    if (e->acc.n_desc)   // same rule as check_sorted_host() in engine.cu
-        for (int f = 0; f < b->n_files; ++f) {
-            bool have = false; int32_t last = 0;
-            for (int64_t i = b->file_start[f]; i < b->file_start[f + 1]; ++i) {
-                if (e->state[(size_t)i] != ST_KEEP) continue;
-                if (have && e->desc[(size_t)i].rpos < last) { e->err = cf->mode == B200_MODE_DEPTH ? "Data is not position sorted" : "The input is not sorted (reads out of order)"; return -3; }
-                have = true; last = e->desc[(size_t)i].rpos;
-            }
-        }
-    const int32_t max_rend = e->acc.n_kept ? e->acc.max_rend : 0;
-    int64_t wend = cf->end - e->win_base, cov = max_rend > 0 ? max_rend : 0;
-    if (cov > wend) cov = wend;
-    int64_t allc = std::min<int64_t>(cf->end, b->tid_len) - e->win_base; if (allc < 0) allc = 0;
-    e->ncols_cov = cov; e->ncols_all = allc; e->ncols_max = (int32_t)std::max(cov, allc);
+    if (e->acc.n_desc)
+        if (const char *msg = unsorted_error(*cf, e->desc.data(), e->state.data(), b->file_start, b->n_files)) { e->err = msg; return -3; }
+    const ColDomain dom = column_domain(*cf, e->win_base, e->acc.n_kept ? e->acc.max_rend : 0, b->tid_len);
+    e->ncols_cov = dom.cov; e->ncols_all = dom.all; e->ncols_max = (int32_t)dom.max();
     e->n_groups = (e->ncols_max + 31) / 32 + 1;
     int max_range = 0;
     build_ranges(e, &max_range);
-    if (cf->mode != B200_MODE_DEPTH && cf->max_depth > 0 && 2LL * max_range + 1 > (int64_t)cf->max_depth) {
-        bool changed = false;
-        for (int f = 0; f < b->n_files; ++f) {
-            std::priority_queue<int32_t, std::vector<int32_t>, std::greater<int32_t>> ends;
-            bool have = false; int32_t pp = 0;
-            for (int64_t i = b->file_start[f]; i < b->file_start[f + 1]; ++i) {
-                if (e->state[(size_t)i] != ST_KEEP) continue;
-                const int32_t pos = e->desc[(size_t)i].rpos, end = pos + e->rlen[(size_t)i];
-                if (have && !(b->rbits && (b->rbits[i] & B200_RB_MAXDEPTH_SEEN))) {   // verdicts of earlier windows stand
-                    while (!ends.empty() && ends.top() < pp) ends.pop();
-                    if (pos == pp && (int64_t)ends.size() + 1 > (int64_t)cf->max_depth) { e->state[(size_t)i] = ST_MAXDROP; changed = true; continue; }
-                }
-                ends.push(end); have = true; pp = pos;
-            }
-        }
-        if (changed) {
-            for (int64_t i = 0; i < n; ++i) if (e->state[(size_t)i] == ST_MAXDROP) { e->desc[(size_t)i].rend = e->desc[(size_t)i].rpos; e->endv[(size_t)i] = INT32_MIN; }
-            build_ranges(e, &max_range);
-        }
+    if (cf->mode != B200_MODE_DEPTH && cf->max_depth > 0 && 2LL * max_range + 1 > (int64_t)cf->max_depth &&
+        apply_max_depth(e->desc.data(), e->rlen.data(), b->rbits, e->state.data(), b->file_start, b->n_files, cf->max_depth)) {
+        for (int64_t i = 0; i < n; ++i) if (e->state[(size_t)i] == ST_MAXDROP) { e->desc[(size_t)i].rend = e->desc[(size_t)i].rpos; e->endv[(size_t)i] = INT32_MIN; }
+        build_ranges(e, &max_range);
     }
     e->has_clip = false;
     if (cf->mode == B200_MODE_DEPTH && cf->d_remove_overlaps && b->depth_clip) {
         e->clip.assign((size_t)n + 1, INT32_MIN);
-        for (int64_t i = 0; i < n; ++i) {
-            int64_t rel = b->depth_clip[i] ? b->depth_clip[i] - e->win_base : (int64_t)INT32_MIN;
-            if (rel > INT32_MAX) rel = INT32_MAX;
-            if (rel < INT32_MIN) rel = INT32_MIN;
-            e->clip[(size_t)i] = (int32_t)rel;
-        }
+        for (int64_t i = 0; i < n; ++i) e->clip[(size_t)i] = window_clip(b->depth_clip[i], e->win_base);
         e->has_clip = true;
     } else if (b->prev_same_name && ((cf->mode == B200_MODE_MPILEUP && cf->overlaps) || (cf->mode == B200_MODE_DEPTH && cf->d_remove_overlaps))) {
         e->next.assign((size_t)n + 1, -1);
