@@ -95,10 +95,15 @@ typedef struct {
                                  rule, bam_plcmd.c:550-554,609): leave it out of the coverage read statistics (coverage.c:185-193) */
 /* The max-depth rule of bam_plp_push depends on every read pushed before: a driver that cuts a reference sequence into
  * windows stages the reads that reach a window from the left again and hands over the verdicts the previous window made
- * (b200_fetch_mapq_keep: 2 = kept, 3 = dropped).  A SEEN read is not judged again: kept, it counts as buffered and as the
+ * (B200_RB_MAXDEPTH_OF below).  A SEEN read is not judged again: kept, it counts as buffered and as the
  * previous read; dropped, it takes no part.  Only reads without SEEN are judged. */
 #define B200_RB_MAXDEPTH_SEEN 16   /* the read's max-depth verdict was made in an earlier window */
 #define B200_RB_MAXDEPTH_DROP 32   /* ... and that verdict was a drop */
+#define B200_KEEP_KEPT    2        /* b200_fetch_mapq_keep state: the read reaches the pileup */
+#define B200_KEEP_MAXDROP 3        /* ... the max-depth rule dropped it (lower states: a filter did, before the rule) */
+/* the carry bits of a b200_fetch_mapq_keep state: 0 for a read the max-depth rule never judged */
+#define B200_RB_MAXDEPTH_OF(keep) ((keep) == B200_KEEP_KEPT ? B200_RB_MAXDEPTH_SEEN : \
+                                   (keep) == B200_KEEP_MAXDROP ? (B200_RB_MAXDEPTH_SEEN | B200_RB_MAXDEPTH_DROP) : 0)
 
 /* ---- read-level configuration (what happens before a read is pushed) ---- */
 typedef enum { B200_MODE_MPILEUP = 0, B200_MODE_DEPTH = 1, B200_MODE_COVERAGE = 2 } b200_mode_t;

@@ -224,47 +224,27 @@ __global__ void k_scan_max(const int32_t *in, int32_t *out, int64_t n, uint64_t 
     for (int j = 0; j < IPT; ++j) if (base + j < n) out[base + j] = max(pre, v[j]);
 }
 
-// per 32-column group: the [lo,hi) slice of each file's reads that can cover it.
-// lo is the later of (a) the first read whose running max end exceeds the group start and
-// (b) the first read starting within kReach columns of it; reads before (b) that still
-// reach the group are listed separately (k_ovf_*), so one spliced read cannot widen the
-// slice of every group under it.
+// per 32-column group: the [lo,hi) slice of each file's reads that can cover it (plp_stage.h group_slice)
 __global__ void k_ranges(const ReadDesc *desc, const int32_t *pmax, const int64_t *file_start, int n_files,
                          int32_t n_groups, int32_t *glo, int32_t *ghi, int *max_range)
 {
     int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (int64_t)n_groups * n_files) return;
     const int f = (int)(idx / n_groups), g = (int)(idx % n_groups);
-    const int64_t fs = file_start[f], fe = file_start[f + 1];
-    const int32_t c0 = g * 32, c1 = c0 + 31;
-    int64_t lo = fs, hi = fe;
-    while (lo < hi) { int64_t m = (lo + hi) >> 1; if (pmax[m] > c0) hi = m; else lo = m + 1; }   // first read whose running max end exceeds c0
-    int64_t first = lo;
-    lo = first; hi = fe;
-    while (lo < hi) { int64_t m = (lo + hi) >> 1; if (desc[m].rpos > c0 - kReach) hi = m; else lo = m + 1; }  // first read within reach
-    if (lo > first) first = lo;
-    lo = first; hi = fe;
-    while (lo < hi) { int64_t m = (lo + hi) >> 1; if (desc[m].rpos > c1) hi = m; else lo = m + 1; }  // first read starting beyond c1
-    const int64_t last = lo > first ? lo : first;
+    int64_t first, last;
+    group_slice(desc, pmax, file_start[f], file_start[f + 1], g, first, last);
     glo[idx] = (int32_t)first;
     ghi[idx] = (int32_t)last;
     atomicMax(max_range, (int)(last - first));
 }
 
-// far-reaching reads: read i is listed for group g when 32g >= rpos_i + kReach and 32g < rend_i
-__device__ __forceinline__ void ovf_span(const ReadDesc &d, int32_t n_groups, int32_t &g0, int32_t &g1)
-{
-    const int64_t a = (int64_t)d.rpos + kReach;
-    g0 = (int32_t)(a <= 0 ? 0 : (a + 31) >> 5);
-    g1 = d.rend > 0 ? (d.rend - 1) >> 5 : -1;
-    if (g1 >= n_groups) g1 = n_groups - 1;
-}
+// far-reaching reads per group (plp_stage.h ovf_span): counts, then the lists
 __global__ void k_ovf_count(const ReadDesc *desc, const int64_t *file_start, int n_files, int64_t n, int32_t n_groups, uint32_t *cnt)
 {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const ReadDesc d = desc[i];
-    if ((int64_t)d.rend - d.rpos <= kReach) return;
+    if (!far_reaching(d)) return;
     int f = 0; while (f + 1 < n_files && i >= file_start[f + 1]) ++f;
     int32_t g0, g1; ovf_span(d, n_groups, g0, g1);
     for (int32_t g = g0; g <= g1; ++g) atomicAdd(&cnt[(int64_t)f * n_groups + g], 1u);
@@ -275,7 +255,7 @@ __global__ void k_ovf_fill(const ReadDesc *desc, const int64_t *file_start, int 
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const ReadDesc d = desc[i];
-    if ((int64_t)d.rend - d.rpos <= kReach) return;
+    if (!far_reaching(d)) return;
     int f = 0; while (f + 1 < n_files && i >= file_start[f + 1]) ++f;
     int32_t g0, g1; ovf_span(d, n_groups, g0, g1);
     for (int32_t g = g0; g <= g1; ++g) {
@@ -393,36 +373,11 @@ __global__ void __launch_bounds__(TILE) k_mpileup_write(MpFmt fmt, const uint32_
 #include "mpileup_ss.cuh"
 #include "mpileup_ent.cuh"
 
-// depth rows "name\tpos(\tdepth)*\n" (bam2depth.c:234-244)
 struct DpFmt {
     View v; DpConf cf;
     struct State { int32_t d0; };
-    __device__ __forceinline__ uint32_t size(int32_t c, State &s) const
-    {
-        bool any = false; uint32_t body = 0;
-        for (int f = 0; f < v.n_files; ++f) {
-            DpCol o; dp_file_column(v, cf, f, c >> 5, c, o);
-            if (f == 0) s.d0 = o.depth;
-            any |= o.spanned;
-            body += 1 + (uint32_t)ndigits((uint64_t)o.depth);
-        }
-        if (!any && !(cf.all && c < v.ncols_all)) return 0;
-        if (!bed_pass(v, c)) return 0;
-        return (uint32_t)v.name_len + 1 + (uint32_t)ndigits((uint64_t)(v.win_base + c + 1)) + body + 1;
-    }
-    __device__ __forceinline__ void write(int32_t c, const State &s, char *p) const
-    {
-        for (int i = 0; i < v.name_len; ++i) *p++ = v.name[i];
-        *p++ = '\t';
-        p += put_u64(p, (uint64_t)(v.win_base + c + 1));
-        for (int f = 0; f < v.n_files; ++f) {
-            int32_t d = s.d0;
-            if (f) { DpCol o; dp_file_column(v, cf, f, c >> 5, c, o); d = o.depth; }
-            *p++ = '\t';
-            p += put_u64(p, (uint64_t)d);
-        }
-        *p = '\n';
-    }
+    __device__ __forceinline__ uint32_t size(int32_t c, State &s) const { return dp_line_size(v, cf, c >> 5, c, s.d0); }
+    __device__ __forceinline__ void write(int32_t c, const State &s, char *p) const { dp_line_write(v, cf, c >> 5, c, s.d0, p); }
 };
 
 __global__ void __launch_bounds__(TILE) k_depth_size(DpFmt fmt, uint32_t *len, DpFmt::State *st, uint32_t *tile_total)
@@ -440,11 +395,7 @@ __global__ void __launch_bounds__(256) k_coverage(View v, int32_t min_baseQ, int
 {
     const int32_t c = (int32_t)(blockIdx.x * blockDim.x + threadIdx.x);
     unsigned long long a[5] = {0, 0, 0, 0, 0};
-    if (c < v.ncols) {
-        CvCol o; cv_column(v, min_baseQ, c >> 5, c, o);
-        a[4] = o.missing;
-        if (o.count_base && o.depth >= (uint32_t)min_depth) { a[0] = 1; a[1] = o.depth; a[2] = o.sum_bq; a[3] = o.qbases; }
-    }
+    if (c < v.ncols) cv_sums(v, min_baseQ, min_depth, c, a);
     __shared__ unsigned long long s[5][8];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
 #pragma unroll
@@ -467,41 +418,23 @@ __global__ void __launch_bounds__(256) k_coverage_hist(View v, int32_t min_baseQ
 {
     const int32_t c = (int32_t)(blockIdx.x * blockDim.x + threadIdx.x);
     if (c >= v.ncols) return;
-    CvCol o; cv_column(v, min_baseQ, c >> 5, c, o);
-    const uint32_t add = plot_depth ? o.depth : ((o.count_base && o.depth >= (uint32_t)min_depth) ? 1u : 0u);
+    const uint32_t add = cv_hist_add(v, min_baseQ, min_depth, plot_depth, c);
     if (!add) return;
     const int64_t bin = ((int64_t)c - beg_rel) / bin_width;
     if (bin >= 0 && bin < n_bins) atomicAdd(&hist[bin], add);
 }
 
-// bedcov column reducers (bedcov.c:316-331) over the staged window, per input file: sum of the per-column depth (optionally
-// without deletions / reference skips) and the number of columns at or above a depth threshold.  A column takes part when
-// the multi-file iterator would return it, i.e. when any file has a read over it.
+// bedcov column reducers (plp_core.h bc_*) over the staged window, per input file: sum of the per-column depth (optionally
+// without deletions / reference skips) and the number of columns at or above a depth threshold
 __global__ void __launch_bounds__(256) k_bedcov(View v, int skip_dn, int min_depth, unsigned long long *sums /* [n_files][2] */)
 {
     const int32_t c = (int32_t)(blockIdx.x * blockDim.x + threadIdx.x);
     const bool live = c < v.ncols;
     bool any = false;
-    if (live)
-        for (int f = 0; f < v.n_files && !any; ++f) {
-            const ReadRange rr = read_range(v, f, c >> 5);
-            for (int32_t t_ = 0; t_ < rr.n && !any; ++t_) { const ReadDesc d = load_hot(v.desc + range_at(rr, t_)); any = (uint32_t)(c - d.rpos) < (uint32_t)(d.rend - d.rpos); }
-        }
+    if (live) any = bc_column_live(v, c >> 5, c);
     for (int f = 0; f < v.n_files; ++f) {
         unsigned long long pd = 0, ge = 0;
-        if (live && any) {
-            const ReadRange rr = read_range(v, f, c >> 5);
-            int32_t np = 0, m = 0;
-            for (int32_t t_ = 0; t_ < rr.n; ++t_) {
-                const int32_t i = range_at(rr, t_);
-                ReadDesc d = load_hot(v.desc + i);
-                if ((uint32_t)(c - d.rpos) >= (uint32_t)(d.rend - d.rpos)) continue;
-                ++np;
-                if (skip_dn && !(d.fl & RD_SIMPLE)) { load_cold(d, v.desc + i); Ent e; resolve(v, d, c, e); if (e.is_del || e.is_refskip) ++m; }
-            }
-            pd = (unsigned long long)(np - m);
-            ge = (min_depth >= 0 && np - m >= min_depth) ? 1ull : 0ull;
-        }
+        if (live && any) bc_file_column(v, skip_dn, min_depth, f, c >> 5, c, pd, ge);
         for (int o = 16; o; o >>= 1) { pd += __shfl_xor_sync(0xffffffffu, pd, o); ge += __shfl_xor_sync(0xffffffffu, ge, o); }
         if ((threadIdx.x & 31) == 0) { if (pd) atomicAdd(&sums[2 * f], pd); if (ge) atomicAdd(&sums[2 * f + 1], ge); }
     }
@@ -529,15 +462,8 @@ __global__ void k_entries_fill(View v, int f, int32_t c0, const uint64_t *col_of
         const int32_t i = range_at(rr, t_);
         const ReadDesc d = v.desc[i];
         if (c < d.rpos || c >= d.rend) continue;
-        Ent e; resolve(v, d, c, e);
-        if (e.k < 0) {   // simple read: the op index of its match
-            const uint32_t *cg = v.cigar + d.cig_off; int k = 0;
-            while (!is_mop(cg[k] & 0xf)) ++k;
-            e.k = k;
-        }
         b200_pileup1_t p;
-        p.read = i; p.qpos = e.qpos; p.indel = e.indel; p.cigar_ind = e.k;
-        p.is_del = e.is_del; p.is_head = e.is_head; p.is_tail = e.is_tail; p.is_refskip = e.is_refskip;
+        pileup1_of(v, d, i, c, p);
         *o++ = p;
     }
 }
@@ -727,8 +653,7 @@ static int apply_maxcnt_host(b200_engine *e, int64_t n, int maxcnt)
 __global__ void k_apply_maxdrop(const uint8_t *state, ReadDesc *desc, int32_t *endv, int64_t n)
 {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    if (state[i] == ST_MAXDROP) { desc[i].rend = desc[i].rpos; endv[i] = INT32_MIN; }
+    if (i < n) apply_maxdrop(state, desc, endv, i);
 }
 
 static int stage_device(b200_engine *e, b200_stage_stats_t *stats);
@@ -854,9 +779,8 @@ static int stage_device(b200_engine *e, b200_stage_stats_t *stats)
     // ---- column domain
     {
         const ColDomain d = column_domain(*cf, e->win_base, e->max_rend, e->tid_len);
-        e->ncols_cov = d.cov; e->ncols_all = d.all;
         if (d.max() >= (1LL << 31) - 4096) { snprintf(e->err, sizeof e->err, "window too wide (%lld columns)", (long long)d.max()); return -1; }
-        e->ncols_max = (int32_t)d.max();
+        e->cols = d; e->ncols_max = (int32_t)d.max();
     }
     e->n_groups = (e->ncols_max + 31) / 32 + 1;
     ENSURE(glo, (size_t)e->n_groups * e->n_files + 1); ENSURE(ghi, (size_t)e->n_groups * e->n_files + 1);
@@ -864,8 +788,7 @@ static int stage_device(b200_engine *e, b200_stage_stats_t *stats)
     int max_range = 0;
     if (n > 0) {
         if (build_ranges(e, &max_range)) return -1;
-        // max-depth rule (bam_plp_push): only reachable when some column can hold > maxcnt reads
-        bool may_fire = cf->mode != B200_MODE_DEPTH && cf->max_depth > 0 && 2LL * max_range + 1 > (int64_t)cf->max_depth;
+        bool may_fire = max_depth_may_fire(*cf, max_range);
         if (may_fire) {   // the slice bound is loose (deep amplicons): exact count on the device before falling back to the host sweep
             int mb = 0;
             if (max_buffered_reads(e, &mb)) return -1;
@@ -902,7 +825,7 @@ static int stage_device(b200_engine *e, b200_stage_stats_t *stats)
     if (stats) {
         stats->n_kept = (int64_t)ha.n_kept; stats->n_kept_in_window = (int64_t)ha.n_kept_in_window;
         stats->n_reads = ha.n_reads; stats->n_selected_reads = ha.n_selected; stats->summed_mapq = ha.summed_mapq;
-        stats->out_bound = e->text_bound(27, 1);
+        stats->out_bound = any_text_bound(e->totals(e->ncols_max));
         stats->n_cols = e->ncols_max;
     }
     return 0;
@@ -962,7 +885,7 @@ int build_ranges(b200_engine *e, int *max_range)
     int mx[2] = {0, 0};                        // widest slice, longest far-reaching list
     CK(cudaMemcpyAsync(mx, e->d_misc + 1, sizeof mx, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
-    *max_range = mx[0] + mx[1];                // no column holds more reads than this
+    *max_range = column_read_bound(mx[0], mx[1]);
     ENSURE(ovf_idx, (size_t)n_ovf + 1);
     if (n_ovf > 0) {
         CK(cudaMemsetAsync(e->ovf_cnt, 0, ((size_t)tot + 1) * 4, e->stream));
@@ -982,8 +905,7 @@ static void fill_view(b200_engine *e, View &v, const int64_t *bed_beg, const int
     v.n_files = e->n_files; v.file_start = e->file_start;
     v.tile_lo = e->glo; v.tile_hi = e->ghi; v.ovf_off = e->ovf_off; v.ovf_idx = e->ovf_idx; v.n_tiles = e->n_groups; v.tile_cols = 32;
     v.win_base = e->win_base;
-    v.ncols_all = all ? (int32_t)e->ncols_all : 0;
-    v.ncols = (int32_t)(all ? std::max(e->ncols_cov, e->ncols_all) : e->ncols_cov);
+    v.ncols_all = e->cols.ncols_all(all); v.ncols = e->cols.ncols(all);
     v.name = e->dname; v.name_len = (int32_t)e->name.size();
     v.bed_beg = bed_beg; v.bed_end = bed_end; v.n_bed = n_bed; v.bed_active = bed_active;
     v.n_x = 0; v.x_stride = 0; v.x_off = nullptr; v.x_dat = nullptr; memset(v.x_sep, 0, sizeof v.x_sep);
@@ -1041,22 +963,10 @@ static int run_text(b200_engine *e, KS k_size, KW k_write, const Fmt &fmt, uint6
     return 0;
 }
 
-static uint64_t mpileup_bound(const b200_engine *e, const b200_mpileup_conf_t *c)
+extern "C" uint64_t b200_mpileup_text_bound(const b200_engine_t *e, const b200_mpileup_conf_t *c)
 {
-    const int per = 2 + (c->out_mapq ? 1 : 0) + (c->out_qpos ? 12 : 0) + (c->out_qpos5 ? 13 : 0);
-    uint64_t b = e->text_bound(per, 1 + 2 * (3 + c->n_star_cols));
-    if (c->n_x > 0 && c->x_off) {   // host columns: every (read, column) entry can add the read's strings + separators
-        uint64_t worst = 0;
-        for (int64_t i = 0; i < e->n; ++i) {
-            uint64_t w = 0;
-            for (int k = 0; k < c->n_x; ++k) { const uint32_t *o = c->x_off + (size_t)k * ((size_t)e->n + 1) + (size_t)i; w += (uint64_t)(o[1] - o[0]) + 1; }
-            worst = std::max(worst, w);
-        }
-        b += (uint64_t)e->sum_rlen * worst;
-    }
-    return b;
+    return (e && e->staged && c) ? mpileup_text_bound(e->totals(e->ncols_max), *c) : 0;
 }
-extern "C" uint64_t b200_mpileup_text_bound(const b200_engine_t *e, const b200_mpileup_conf_t *c) { return (e && e->staged && c) ? mpileup_bound(e, c) : 0; }
 
 extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c, char *out, size_t out_cap, size_t *out_len)
 {
@@ -1068,8 +978,8 @@ extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c,
     fmt.cf.min_baseQ = c->min_baseQ; fmt.cf.all = c->all; fmt.cf.rev_del = c->rev_del; fmt.cf.no_ins = c->no_ins;
     fmt.cf.no_del = c->no_del; fmt.cf.no_ends = c->no_ends; fmt.cf.out_mapq = c->out_mapq; fmt.cf.out_qpos = c->out_qpos;
     fmt.cf.out_qpos5 = c->out_qpos5; fmt.cf.n_star_cols = c->n_star_cols;
-    const uint64_t bound = mpileup_bound(e, c);
-    if (c->n_x > 0) {   // host columns: upload the per-read string tables, widen the bound by the longest per-read contribution
+    const uint64_t bound = mpileup_text_bound(e->totals(e->ncols_max), *c);
+    if (c->n_x > 0) {   // host columns: upload the per-read string tables
         if (c->n_x > PLP_MAX_X || c->n_x != c->n_star_cols || !c->x_off || (!c->x_dat && c->x_bytes)) { snprintf(e->err, sizeof e->err, "bad host-column tables"); return -1; }
         const size_t n_off = (size_t)c->n_x * ((size_t)e->n + 1);
         H2D(x_off, c->x_off, n_off); H2D(x_dat, c->x_dat, c->x_bytes ? c->x_bytes : 1);
@@ -1160,14 +1070,11 @@ extern "C" int b200_depth_text(b200_engine_t *e, const b200_depth_conf_t *c, cha
     DpFmt fmt;
     fill_view(e, fmt.v, e->bed_beg, e->bed_end, c->n_bed, c->bed_active, c->all);
     fmt.cf.min_qual = c->min_qual; fmt.cf.count_del = c->count_del; fmt.cf.all = c->all;
-    const uint64_t ncols = (uint64_t)fmt.v.ncols;
-    const uint64_t bound = ncols * (e->name.size() + 1 + 20 + (uint64_t)e->n_files * 12 + 1) + 64;
-    return run_text(e, k_depth_size, k_depth_write, fmt, bound, out, out_cap, out_len);
+    return run_text(e, k_depth_size, k_depth_write, fmt, depth_text_bound(e->totals(fmt.v.ncols)), out, out_cap, out_len);
 }
 extern "C" uint64_t b200_depth_text_bound(const b200_engine_t *e)
 {
-    if (!e || !e->staged) return 0;
-    return (uint64_t)e->ncols_max * (e->name.size() + 1 + 20 + (uint64_t)e->n_files * 12 + 1) + 64;
+    return (e && e->staged) ? depth_text_bound(e->totals(e->ncols_max)) : 0;
 }
 
 extern "C" int b200_coverage(b200_engine_t *e, const b200_coverage_conf_t *c, b200_coverage_sums_t *sums)
@@ -1218,7 +1125,7 @@ extern "C" int b200_bedcov(b200_engine_t *e, int32_t skip_del_refskip, int32_t m
     ENSURE(col_off, 2 * nf + 2);
     CK(cudaMemsetAsync(e->col_off, 0, 2 * nf * 8, e->stream));
     CK(cudaEventRecord(e->ev0, e->stream));
-    k_bedcov<<<nblk(v.ncols, 256), 256, 0, e->stream>>>(v, (skip_del_refskip || min_depth >= 0) ? 1 : 0, min_depth, (unsigned long long *)e->col_off); e->launches++;
+    k_bedcov<<<nblk(v.ncols, 256), 256, 0, e->stream>>>(v, skip_del_refskip, min_depth,(unsigned long long *)e->col_off); e->launches++;
     CK(cudaEventRecord(e->ev1, e->stream));
     std::vector<uint64_t> h(2 * nf);
     CK(cudaMemcpyAsync(h.data(), e->col_off, 2 * nf * 8, cudaMemcpyDeviceToHost, e->stream));

@@ -5,7 +5,7 @@
 #include <string>
 #include <vector>
 #include "../../include/b200_pileup.h"
-#include "plp_core.h"
+#include "plp_stage.h"
 
 #define DBUF(type, name) type *name = nullptr; size_t cap_##name = 0
 
@@ -55,7 +55,7 @@ struct b200_engine {
     std::string name;
     b200_stage_conf_t sconf;
     int64_t win_base = 0, ref_beg = 0, ref_n = 0, ref_len = 0;
-    int64_t ncols_cov = 0, ncols_all = 0; int32_t ncols_max = 0, n_groups = 0;
+    plp::ColDomain cols = {0, 0}; int32_t ncols_max = 0, n_groups = 0;
     int64_t acc_n_kept = 0; int32_t max_rend = 0;
     unsigned long long sum_rlen = 0, sum_indel_text = 0, sum_rlen_gen = 0;
     size_t last_out_len = 0;
@@ -63,11 +63,7 @@ struct b200_engine {
     std::vector<int64_t> h_file_start;
     std::vector<int32_t> h_rlen_tmp, h_clip_tmp;
 
-    uint64_t text_bound(int per_entry, int per_file_extra) const
-    {
-        return (uint64_t)sum_rlen * (uint64_t)per_entry + sum_indel_text +
-               (uint64_t)ncols_max * (name.size() + 24 + (uint64_t)n_files * (16 + (uint64_t)per_file_extra)) + 64;
-    }
+    plp::TextTotals totals(int64_t ncols) const { return {sum_rlen, sum_indel_text, n, ncols, (uint64_t)name.size(), n_files}; }
     void free_all()
     {
         void *ps[] = { qual0, mapq0, pos, flag, mapq, l_qseq, n_cigar, cigar_off, qual_off, mtid, mpos, isize, prev, rbits, cigar, seq4, qual,
@@ -77,7 +73,6 @@ struct b200_engine {
     }
 };
 
-namespace plp { struct RawSoA; }
 using plp::RawSoA;
 int build_ranges(b200_engine *e, int *max_range);
 int launch_baq(b200_engine *e, const RawSoA &r, const b200_stage_conf_t &cf);

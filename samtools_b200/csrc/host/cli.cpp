@@ -219,7 +219,7 @@ int64_t max_stacked_records(const std::vector<FileData> &fd, int tid)
     return best;
 }
 // The max-depth verdicts of one contig's records, handed from each window to the next: after a window is staged, every
-// record the engine kept (2) or dropped (3) remembers it, and a later window that stages the record again passes it on.
+// record the engine kept or dropped (B200_KEEP_*) remembers it, and a later window that stages the record again passes it on.
 struct MaxDepthCarry {
     bool on = false;
     std::vector<std::vector<uint8_t>> bits;   // per file, per record of the contig: B200_RB_MAXDEPTH_* or 0
@@ -236,11 +236,8 @@ struct MaxDepthCarry {
         if (!on) return 0;
         keep.resize(staged.size());
         if (!staged.empty() && b200_fetch_mapq_keep(e, nullptr, keep.data(), keep.size()) != 0) return -1;
-        for (size_t k = 0; k < staged.size(); ++k) {
-            uint8_t &b = bits[(size_t)staged[k].first][staged[k].second];
-            if (keep[k] == 2) b = B200_RB_MAXDEPTH_SEEN;
-            else if (keep[k] == 3) b = B200_RB_MAXDEPTH_SEEN | B200_RB_MAXDEPTH_DROP;
-        }
+        for (size_t k = 0; k < staged.size(); ++k)
+            if (const uint8_t b = B200_RB_MAXDEPTH_OF(keep[k])) bits[(size_t)staged[k].first][staged[k].second] = b;
         staged.clear();
         return 0;
     }

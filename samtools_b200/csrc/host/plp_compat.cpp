@@ -165,8 +165,7 @@ static int stage_batch(b200_plp *it)
         std::vector<uint8_t> keep(n);
         if (b200_fetch_mapq_keep(it->eng, nullptr, keep.data(), n) != 0) return -1;
         for (size_t i = 0; i < n; ++i)
-            if (keep[i] == 2) it->batch_md[i] = B200_RB_MAXDEPTH_SEEN;
-            else if (keep[i] == 3) it->batch_md[i] = B200_RB_MAXDEPTH_SEEN | B200_RB_MAXDEPTH_DROP;
+            if (const uint8_t b = B200_RB_MAXDEPTH_OF(keep[i])) it->batch_md[i] = b;
     }
     it->col = 0; it->slab_beg = it->slab_end = 0; it->ent_pos = 0;
     return 0;

@@ -7,7 +7,7 @@
 //   k_mp_entries (mpileup_ent.cuh) one warp per 32 reads, lanes over their bases: a coverage difference array gets
 //                +1/-1 per read, only FAILING bases and special entries touch per-column counters (sparse atomics)
 //   k_ss_scan    prefix sum of the difference array -> n_plp per column
-//   k_ss_cols    per column: cnt = n_plp - fail, seq_len = cnt + extra -> MpFileSz, line length,
+//   k_ss_cols    per column: MpFileSz and line length from the sums (plp_core.h mp_sums_line_size),
 //                128-column tile totals (what the write kernel and the offset scan consume)
 // Equivalent to mp_line_size (the general path); `test_c2_size_properties` checks that both paths agree.
 #pragma once
@@ -41,10 +41,7 @@ __global__ void __launch_bounds__(TILE) k_ss_cols(View v, MpConf cf, const int32
     const int32_t c = (int32_t)blockIdx.x * TILE + (int32_t)threadIdx.x;
     uint32_t len = 0;
     if (c < v.ncols) {
-        MpFileSz s;
-        s.nplp = nplp[c]; s.cnt = s.nplp - (int32_t)fail[c]; s.seq_len = (uint32_t)s.cnt + extra[c]; s.bp_len = 0; s.bp5_len = 0;
-        fsz[c] = s;
-        if ((s.nplp > 0 || (cf.all && c < v.ncols_all)) && bed_pass(v, c)) len = mp_head_len(v, c) + mp_file_section_len(cf, s) + 1;
+        len = mp_sums_line_size(v, cf, c, nplp[c], fail[c], extra[c], fsz + c);
         len_out[c] = len;
     }
     uint32_t x = len;

@@ -14,9 +14,11 @@
 //   mp_file_size/write   column loop per file      bam_plcmd.c:669-797
 //   mp_empty_*           print_empty_pileup        bam_plcmd.c:372-398
 //   dp_*                 add_depth / flush rows    bam2depth.c:209-477
-//   cv_column            coverage reducers         coverage.c:622-660
+//   cv_*                 coverage reducers         coverage.c:622-660
+//   bc_*                 bedcov reducers           bedcov.c:316-331
 #pragma once
 #include <stdint.h>
+#include "../../include/b200_pileup.h"
 
 #if defined(__CUDACC__)
 #define PLP_HD __host__ __device__ __forceinline__
@@ -689,6 +691,17 @@ PLP_HD void mp_line_write(const View &v, const MpConf &cf, int tile, int32_t c, 
     *p = '\n';
 }
 
+// The same for one file without -O columns, from order-free sums (the default path, mpileup_ss.cuh): nplp reads over the
+// column, fail of them below -Q, extra bytes of their "^"+mapq, "$" and indel text.  The state goes to *s0.
+PLP_HD uint32_t mp_sums_line_size(const View &v, const MpConf &cf, int32_t c, int32_t nplp, uint32_t fail, uint32_t extra, MpFileSz *s0)
+{
+    MpFileSz s;
+    s.nplp = nplp; s.cnt = s.nplp - (int32_t)fail; s.seq_len = (uint32_t)s.cnt + extra; s.bp_len = 0; s.bp5_len = 0;
+    *s0 = s;
+    if ((s.nplp > 0 || (cf.all && c < v.ncols_all)) && bed_pass(v, c)) return mp_head_len(v, c) + mp_file_section_len(cf, s) + 1;
+    return 0;
+}
+
 // ---- entry strings: the default single-file mpileup path (mpileup_ent.cuh) ------------------
 // pileup_seq (bam_plcmd.c:54-169) emits, for almost every (read, column), ONE sequence character and ONE
 // quality character.  A read-major pass (lanes along the read: wide coalesced loads, no per-column
@@ -966,6 +979,78 @@ PLP_HD void dp_file_column(const View &v, const DpConf &cf, int f, int tile, int
     }
 }
 
+// depth row "name\tpos(\tdepth)*\n" of column c (bam2depth.c:234-244); 0: the column is not reported.  d0 keeps the first
+// file's depth for the writer.
+PLP_HD uint32_t dp_line_size(const View &v, const DpConf &cf, int tile, int32_t c, int32_t &d0)
+{
+    bool any = false; uint32_t body = 0;
+    for (int f = 0; f < v.n_files; ++f) {
+        DpCol o; dp_file_column(v, cf, f, tile, c, o);
+        if (f == 0) d0 = o.depth;
+        any |= o.spanned;
+        body += 1 + (uint32_t)ndigits((uint64_t)o.depth);
+    }
+    if (!any && !(cf.all && c < v.ncols_all)) return 0;
+    if (!bed_pass(v, c)) return 0;
+    return (uint32_t)v.name_len + 1 + (uint32_t)ndigits((uint64_t)(v.win_base + c + 1)) + body + 1;
+}
+PLP_HD void dp_line_write(const View &v, const DpConf &cf, int tile, int32_t c, int32_t d0, char *p)
+{
+    for (int i = 0; i < v.name_len; ++i) *p++ = v.name[i];
+    *p++ = '\t';
+    p += put_u64(p, (uint64_t)(v.win_base + c + 1));
+    for (int f = 0; f < v.n_files; ++f) {
+        int32_t d = d0;
+        if (f) { DpCol o; dp_file_column(v, cf, f, tile, c, o); d = o.depth; }
+        *p++ = '\t';
+        p += put_u64(p, (uint64_t)d);
+    }
+    *p = '\n';
+}
+
+// ---- bedcov (bedcov.c:316-331) ------------------------------------------------
+// A column takes part when the multi-file iterator would return it, i.e. when any file has a read over it.
+PLP_HD bool bc_column_live(const View &v, int tile, int32_t c)
+{
+    bool any = false;
+    for (int f = 0; f < v.n_files && !any; ++f) {
+        const ReadRange rr = read_range(v, f, tile);
+        for (int32_t t_ = 0; t_ < rr.n && !any; ++t_) { const ReadDesc d = load_hot(v.desc + range_at(rr, t_)); any = (uint32_t)(c - d.rpos) < (uint32_t)(d.rend - d.rpos); }
+    }
+    return any;
+}
+// what file f adds at a live column: its depth and whether that depth reaches min_depth (min_depth < 0: never).  Deletions
+// and reference skips do not count with skip_dn or with a min_depth.
+PLP_HD void bc_file_column(const View &v, int skip_dn, int min_depth, int f, int tile, int32_t c, unsigned long long &depth, unsigned long long &ge)
+{
+    skip_dn = skip_dn || min_depth >= 0;
+    const ReadRange rr = read_range(v, f, tile);
+    int32_t np = 0, m = 0;
+    for (int32_t t_ = 0; t_ < rr.n; ++t_) {
+        const int32_t i = range_at(rr, t_);
+        ReadDesc d = load_hot(v.desc + i);
+        if ((uint32_t)(c - d.rpos) >= (uint32_t)(d.rend - d.rpos)) continue;
+        ++np;
+        if (skip_dn && !(d.fl & RD_SIMPLE)) { load_cold(d, v.desc + i); Ent e; resolve(v, d, c, e); if (e.is_del || e.is_refskip) ++m; }
+    }
+    depth = (unsigned long long)(np - m);
+    ge = (min_depth >= 0 && np - m >= min_depth) ? 1ull : 0ull;
+}
+
+// ---- pileup entries (the iterator tier) -----------------------------------------
+// the bam_pileup1_t fields of read i at column c; a simple read's cigar_ind is the op index of its match
+PLP_HD void pileup1_of(const View &v, const ReadDesc &d, int32_t i, int32_t c, b200_pileup1_t &p)
+{
+    Ent e; resolve(v, d, c, e);
+    if (e.k < 0) {
+        const uint32_t *cg = v.cigar + d.cig_off; int k = 0;
+        while (!is_mop(cg[k] & 0xf)) ++k;
+        e.k = k;
+    }
+    p.read = i; p.qpos = e.qpos; p.indel = e.indel; p.cigar_ind = e.k;
+    p.is_del = e.is_del; p.is_head = e.is_head; p.is_tail = e.is_tail; p.is_refskip = e.is_refskip;
+}
+
 // ---- coverage (coverage.c:622-660) --------------------------------------------
 struct CvCol { uint32_t depth; uint32_t qbases; uint64_t sum_bq; uint32_t missing; bool count_base; };
 
@@ -998,6 +1083,22 @@ PLP_HD void cv_column(const View &v, int32_t min_baseQ, int tile, int32_t c, CvC
         }
         if (dpos > 0) { o.count_base = true; o.depth += (uint32_t)dpos; }
     }
+}
+
+// What column c adds to b200_coverage_sums_t, in its field order: n_covered_bases, summed_coverage, summed_baseQ,
+// quality_bases, missing_qual.  A column counts as covered when some file has a base there and the depth reaches
+// --min-depth.
+PLP_HD void cv_sums(const View &v, int32_t min_baseQ, int32_t min_depth, int32_t c, unsigned long long (&a)[5])
+{
+    CvCol o; cv_column(v, min_baseQ, c >> 5, c, o);
+    a[4] = o.missing;
+    if (o.count_base && o.depth >= (uint32_t)min_depth) { a[0] = 1; a[1] = o.depth; a[2] = o.sum_bq; a[3] = o.qbases; }
+}
+// what column c adds to its histogram bin: its depth (plot_depth) or 1 when it counts as covered
+PLP_HD uint32_t cv_hist_add(const View &v, int32_t min_baseQ, int32_t min_depth, int plot_depth, int32_t c)
+{
+    CvCol o; cv_column(v, min_baseQ, c >> 5, c, o);
+    return plot_depth ? o.depth : ((o.count_base && o.depth >= (uint32_t)min_depth) ? 1u : 0u);
 }
 
 }  // namespace plp

@@ -43,7 +43,7 @@ struct StageAcc {   // device-side accumulators (one instance per stage call)
     int max_rend;
 };
 
-enum { ST_DEAD = 0, ST_ALIVE = 1, ST_KEEP = 2, ST_MAXDROP = 3 };
+enum { ST_DEAD = 0, ST_ALIVE = 1, ST_KEEP = B200_KEEP_KEPT, ST_MAXDROP = B200_KEEP_MAXDROP };
 
 // geometry + filters that precede BAQ (bam_plcmd.c:413-445; bam2depth.c:552-570; coverage.c:185-190)
 PLP_HD void stage_prep1(const RawSoA &r, const b200_stage_conf_t &cf, int64_t i, uint8_t *state, int32_t *rlen_out, StageAcc *acc)
@@ -226,6 +226,51 @@ PLP_HD void stage_build_desc(const RawSoA &r, const b200_stage_conf_t &cf, int64
         PLP_ADD64(&acc->sum_indel_text, it);
         PLP_MAX32(&acc->max_rend, d.rend);
     }
+}
+
+
+// ---- per-group read slices --------------------------------------------------
+// The reads of file [fs,fe) that can cover 32-column group g: the slice [first,last).  first is the later of (a) the first
+// read whose running max end (pmax: prefix max of endv) exceeds the group start and (b) the first read starting within
+// kReach columns of it; reads before (b) that still reach the group are far-reaching and listed separately (below), so one
+// spliced read cannot widen the slice of every group under it.  last: the first read starting beyond the group.
+PLP_HD void group_slice(const ReadDesc *desc, const int32_t *pmax, int64_t fs, int64_t fe, int32_t g, int64_t &first, int64_t &last)
+{
+    const int32_t c0 = g * 32, c1 = c0 + 31;
+    int64_t lo = fs, hi = fe;
+    while (lo < hi) { int64_t m = (lo + hi) >> 1; if (pmax[m] > c0) hi = m; else lo = m + 1; }   // first read whose running max end exceeds c0
+    first = lo;
+    lo = first; hi = fe;
+    while (lo < hi) { int64_t m = (lo + hi) >> 1; if (desc[m].rpos > c0 - kReach) hi = m; else lo = m + 1; }  // first read within reach
+    if (lo > first) first = lo;
+    lo = first; hi = fe;
+    while (lo < hi) { int64_t m = (lo + hi) >> 1; if (desc[m].rpos > c1) hi = m; else lo = m + 1; }  // first read starting beyond c1
+    last = lo > first ? lo : first;
+}
+
+// far-reaching reads: read i is listed for group g when 32g >= rpos_i + kReach and 32g < rend_i, i.e. for groups [g0, g1]
+PLP_HD bool far_reaching(const ReadDesc &d) { return (int64_t)d.rend - d.rpos > kReach; }
+PLP_HD void ovf_span(const ReadDesc &d, int32_t n_groups, int32_t &g0, int32_t &g1)
+{
+    const int64_t a = (int64_t)d.rpos + kReach;
+    g0 = (int32_t)(a <= 0 ? 0 : (a + 31) >> 5);
+    g1 = d.rend > 0 ? (d.rend - 1) >> 5 : -1;
+    if (g1 >= n_groups) g1 = n_groups - 1;
+}
+
+// no column holds more reads of one file than the widest slice plus the longest far-reaching list
+PLP_HD int column_read_bound(int widest_slice, int longest_list) { return widest_slice + longest_list; }
+
+// the max-depth rule of bam_plp_push can only fire when a column may hold more than max_depth reads (see DESIGN.md)
+PLP_HD bool max_depth_may_fire(const b200_stage_conf_t &cf, int column_reads)
+{
+    return cf.mode != B200_MODE_DEPTH && cf.max_depth > 0 && 2LL * column_reads + 1 > (int64_t)cf.max_depth;
+}
+
+// a read the max-depth rule dropped covers no column and leaves the slices
+PLP_HD void apply_maxdrop(const uint8_t *state, ReadDesc *desc, int32_t *endv, int64_t i)
+{
+    if (state[i] == ST_MAXDROP) { desc[i].rend = desc[i].rpos; endv[i] = INT32_MIN; }
 }
 
 
@@ -498,9 +543,12 @@ inline int32_t window_clip(int64_t clip, int64_t win_base)
 
 // Columns of a staged window, relative to its start: `cov` up to the end of the kept reads (max_rend, 0 without kept
 // reads), `all` up to the contig's end (the -a rows); both cut at the region's end.
+// A View over the window formats ncols(all) columns; with -a the first ncols_all(all) of them print even when empty.
 struct ColDomain {
     int64_t cov, all;
     int64_t max() const { return cov > all ? cov : all; }
+    int32_t ncols(int with_all) const { return (int32_t)(with_all ? max() : cov); }
+    int32_t ncols_all(int with_all) const { return with_all ? (int32_t)all : 0; }
 };
 inline ColDomain column_domain(const b200_stage_conf_t &cf, int64_t win_base, int32_t max_rend, int64_t tid_len)
 {
@@ -510,6 +558,47 @@ inline ColDomain column_domain(const b200_stage_conf_t &cf, int64_t win_base, in
     d.all = (cf.end < tid_len ? cf.end : tid_len) - win_base;
     if (d.all < 0) d.all = 0;
     return d;
+}
+
+// Upper bounds of the text a staged window can produce, from its totals.  Callers size their buffers with them
+// (b200_*_text_bound), and a text that comes out longer is an internal error.
+struct TextTotals {
+    unsigned long long sum_rlen, sum_indel_text;   // StageAcc: reference span of the kept reads, bound of their indel text
+    int64_t n_reads;
+    int64_t ncols;                                  // columns a line may be printed for
+    uint64_t name_len;
+    int32_t n_files;
+};
+// mpileup: per (read, column) entry the base, its quality and the -s / -O / --output-BP-5 values; per indel its text; per
+// line the name, position, reference base and separators; per file the count, the empty-entry place holders and the "\t*"
+// of the host columns.  Host columns add, per entry, the longest set of strings a read prints in them.
+inline uint64_t mpileup_text_bound(const TextTotals &t, const b200_mpileup_conf_t &c)
+{
+    const uint64_t per_entry = 2 + (c.out_mapq ? 1 : 0) + (c.out_qpos ? 12 : 0) + (c.out_qpos5 ? 13 : 0);
+    const uint64_t per_file = 16 + 1 + 2 * (3 + (uint64_t)c.n_star_cols);
+    uint64_t b = (uint64_t)t.sum_rlen * per_entry + t.sum_indel_text + (uint64_t)t.ncols * (t.name_len + 24 + (uint64_t)t.n_files * per_file) + 64;
+    if (c.n_x > 0 && c.x_off) {
+        uint64_t worst = 0;
+        for (int64_t i = 0; i < t.n_reads; ++i) {
+            uint64_t w = 0;
+            for (int k = 0; k < c.n_x; ++k) { const uint32_t *o = c.x_off + (size_t)k * ((size_t)t.n_reads + 1) + (size_t)i; w += (uint64_t)(o[1] - o[0]) + 1; }
+            if (w > worst) worst = w;
+        }
+        b += (uint64_t)t.sum_rlen * worst;
+    }
+    return b;
+}
+// depth: every row is the name, a tab, the position (<= 20 digits), a tab and a depth (<= 11 characters) per file, a newline
+inline uint64_t depth_text_bound(const TextTotals &t)
+{
+    return (uint64_t)t.ncols * (t.name_len + 1 + 20 + (uint64_t)t.n_files * 12 + 1) + 64;
+}
+// b200_stage_stats_t::out_bound: mpileup with every column the device formats itself (which also bounds the depth rows)
+inline uint64_t any_text_bound(const TextTotals &t)
+{
+    b200_mpileup_conf_t c = {};
+    c.out_mapq = c.out_qpos = c.out_qpos5 = 1;
+    return mpileup_text_bound(t, c);
 }
 
 

@@ -3,7 +3,11 @@
 // Implements the C ABI of include/b200_pileup.h by stepping the very same
 // __host__ __device__ per-read / per-column functions the CUDA kernels call
 // (samtools_b200/csrc/plp_core.h, plp_stage.h) in a plain single-threaded
-// loop.  It exists so that the column arithmetic and the host drivers can be
+// loop: the read stage, the per-group read slices and far-reaching lists, the
+// max-depth gate, every per-column formatter and reducer (mpileup and depth
+// rows, order-free line sizes, coverage, bedcov, pileup entries), the View's
+// column counts and the text bounds.  Only the loops, scans and buffers are
+// its own.  It exists so that the column arithmetic and the host drivers can be
 // debugged on a machine without a GPU.  It is built only by
 // tests/emul/build.sh, is never linked into libb200pileup.so or b200samtools,
 // is never used as a fallback, and is not a measured or shipped path.
@@ -28,9 +32,15 @@ struct b200_engine {
     std::vector<int64_t> next, bedb, bede;
     std::string ref;
     StageAcc acc;
-    int64_t win_base = 0, ncols_cov = 0, ncols_all = 0; int32_t ncols_max = 0, n_groups = 0;
+    ColDomain cols = {0, 0};
+    int64_t win_base = 0; int32_t ncols_max = 0, n_groups = 0;
     bool staged = false, has_clip = false;
 };
+
+static TextTotals totals(const b200_engine *e, int64_t ncols)
+{
+    return {e->acc.sum_rlen, e->acc.sum_indel_text, e->b.n_reads, ncols, (uint64_t)e->name.size(), e->b.n_files};
+}
 
 extern "C" {
 const char *b200_version(void) { return "emulation harness (debug only)"; }
@@ -56,7 +66,9 @@ static RawSoA raw(b200_engine *e)
     return r;
 }
 
-static void build_ranges(b200_engine *e, int *max_range)
+// per-group read slices and far-reaching lists: the loops of k_scan_max, k_ranges and k_ovf_* (engine.cu) around the same
+// plp_stage.h rules; returns the bound on the reads of one file over one column
+static int build_ranges(b200_engine *e)
 {
     const b200_batch_t &b = e->b;
     const int64_t n = b.n_reads;
@@ -66,39 +78,29 @@ static void build_ranges(b200_engine *e, int *max_range)
         for (int64_t i = b.file_start[f]; i < b.file_start[f + 1]; ++i) { m = std::max(m, e->endv[(size_t)i]); e->pmax[(size_t)i] = m; }
     }
     e->glo.assign((size_t)e->n_groups * b.n_files + 1, 0); e->ghi = e->glo;
-    *max_range = 0;
+    int widest = 0;
     for (int f = 0; f < b.n_files; ++f)
         for (int g = 0; g < e->n_groups; ++g) {
-            const int64_t fs = b.file_start[f], fe = b.file_start[f + 1];
-            const int32_t c0 = g * 32, c1 = c0 + 31;
-            int64_t lo = fs, hi = fe;
-            while (lo < hi) { int64_t m = (lo + hi) >> 1; if (e->pmax[(size_t)m] > c0) hi = m; else lo = m + 1; }
-            int64_t first = lo;
-            hi = fe;
-            while (lo < hi) { int64_t m = (lo + hi) >> 1; if (e->desc[(size_t)m].rpos > c0 - kReach) hi = m; else lo = m + 1; }
-            if (lo > first) first = lo;
-            lo = first; hi = fe;
-            while (lo < hi) { int64_t m = (lo + hi) >> 1; if (e->desc[(size_t)m].rpos > c1) hi = m; else lo = m + 1; }
-            const int64_t last = std::max(lo, first);
+            int64_t first, last;
+            group_slice(e->desc.data(), e->pmax.data(), b.file_start[f], b.file_start[f + 1], g, first, last);
             e->glo[(size_t)f * e->n_groups + g] = (int32_t)first; e->ghi[(size_t)f * e->n_groups + g] = (int32_t)last;
-            *max_range = std::max(*max_range, (int)(last - first));
+            widest = std::max(widest, (int)(last - first));
         }
-    // far-reaching reads per group (same rule as k_ovf_*)
     std::vector<std::vector<int32_t>> lists((size_t)e->n_groups * b.n_files);
     for (int f = 0; f < b.n_files; ++f)
         for (int64_t i = b.file_start[f]; i < b.file_start[f + 1]; ++i) {
             const ReadDesc &d = e->desc[(size_t)i];
-            if ((int64_t)d.rend - d.rpos <= kReach) continue;
-            const int64_t a = (int64_t)d.rpos + kReach;
-            int32_t g0 = (int32_t)(a <= 0 ? 0 : (a + 31) >> 5), g1 = d.rend > 0 ? (d.rend - 1) >> 5 : -1;
-            if (g1 >= e->n_groups) g1 = e->n_groups - 1;
+            if (!far_reaching(d)) continue;
+            int32_t g0, g1; ovf_span(d, e->n_groups, g0, g1);
             for (int32_t g = g0; g <= g1; ++g) lists[(size_t)f * e->n_groups + g].push_back((int32_t)i);
         }
-    { size_t mo = 0; for (auto &l : lists) mo = std::max(mo, l.size()); *max_range += (int)mo; }
+    size_t longest = 0;
+    for (auto &l : lists) longest = std::max(longest, l.size());
     e->ovf_off.assign(lists.size() + 2, 0); e->ovf_idx.clear();
     for (size_t k = 0; k < lists.size(); ++k) { e->ovf_off[k] = (int32_t)e->ovf_idx.size(); e->ovf_idx.insert(e->ovf_idx.end(), lists[k].begin(), lists[k].end()); }
     e->ovf_off[lists.size()] = (int32_t)e->ovf_idx.size(); e->ovf_off[lists.size() + 1] = (int32_t)e->ovf_idx.size();
     e->ovf_idx.push_back(0);
+    return column_read_bound(widest, (int)longest);
 }
 
 int b200_stage(b200_engine_t *e, const b200_batch_t *b, const b200_stage_conf_t *cf, b200_stage_stats_t *stats)
@@ -126,15 +128,13 @@ int b200_stage(b200_engine_t *e, const b200_batch_t *b, const b200_stage_conf_t 
     for (int64_t i = 0; i < n; ++i) stage_build_desc(r, *cf, i, e->state.data(), e->rlen.data(), e->desc.data(), e->endv.data(), &e->acc, e->win_base, e->cig_x.data(), e->cig_y.data());
     if (e->acc.n_desc)
         if (const char *msg = unsorted_error(*cf, e->desc.data(), e->state.data(), b->file_start, b->n_files)) { e->err = msg; return -3; }
-    const ColDomain dom = column_domain(*cf, e->win_base, e->acc.n_kept ? e->acc.max_rend : 0, b->tid_len);
-    e->ncols_cov = dom.cov; e->ncols_all = dom.all; e->ncols_max = (int32_t)dom.max();
+    e->cols = column_domain(*cf, e->win_base, e->acc.n_kept ? e->acc.max_rend : 0, b->tid_len);
+    e->ncols_max = (int32_t)e->cols.max();
     e->n_groups = (e->ncols_max + 31) / 32 + 1;
-    int max_range = 0;
-    build_ranges(e, &max_range);
-    if (cf->mode != B200_MODE_DEPTH && cf->max_depth > 0 && 2LL * max_range + 1 > (int64_t)cf->max_depth &&
+    if (max_depth_may_fire(*cf, build_ranges(e)) &&
         apply_max_depth(e->desc.data(), e->rlen.data(), b->rbits, e->state.data(), b->file_start, b->n_files, cf->max_depth)) {
-        for (int64_t i = 0; i < n; ++i) if (e->state[(size_t)i] == ST_MAXDROP) { e->desc[(size_t)i].rend = e->desc[(size_t)i].rpos; e->endv[(size_t)i] = INT32_MIN; }
-        build_ranges(e, &max_range);
+        for (int64_t i = 0; i < n; ++i) apply_maxdrop(e->state.data(), e->desc.data(), e->endv.data(), i);
+        build_ranges(e);
     }
     e->has_clip = false;
     if (cf->mode == B200_MODE_DEPTH && cf->d_remove_overlaps && b->depth_clip) {
@@ -159,7 +159,7 @@ int b200_stage(b200_engine_t *e, const b200_batch_t *b, const b200_stage_conf_t 
         memset(stats, 0, sizeof *stats);
         stats->n_kept = (int64_t)e->acc.n_kept; stats->n_kept_in_window = (int64_t)e->acc.n_kept_in_window;
         stats->n_reads = e->acc.n_reads; stats->n_selected_reads = e->acc.n_selected; stats->summed_mapq = e->acc.summed_mapq;
-        stats->out_bound = 0; stats->n_cols = e->ncols_max;
+        stats->out_bound = any_text_bound(totals(e, e->ncols_max)); stats->n_cols = e->ncols_max;
     }
     return 0;
 }
@@ -173,15 +173,15 @@ static void fill_view(b200_engine *e, View &v, const int64_t *bb, const int64_t 
     v.ref_off = b.ref_beg - e->win_base; v.ref_n = b.ref_n; v.ref_len_rel = (v.ref ? b.ref_len : 0) - e->win_base;
     v.n_files = b.n_files; v.file_start = b.file_start; v.tile_lo = e->glo.data(); v.tile_hi = e->ghi.data(); v.ovf_off = e->ovf_off.data(); v.ovf_idx = e->ovf_idx.data();
     v.n_tiles = e->n_groups; v.tile_cols = 32; v.win_base = e->win_base;
-    v.ncols_all = all ? (int32_t)e->ncols_all : 0;
-    v.ncols = (int32_t)(all ? std::max(e->ncols_cov, e->ncols_all) : e->ncols_cov);
-    v.name = e->name.c_str(); v.name_len = (int32_t)e->name.size();
+    v.ncols_all = e->cols.ncols_all(all); v.ncols = e->cols.ncols(all);
+    v.name =e->name.c_str(); v.name_len = (int32_t)e->name.size();
     v.bed_beg = bb; v.bed_end = be; v.n_bed = nb; v.bed_active = active;
     v.n_x = 0; v.x_stride = 0; v.x_off = nullptr; v.x_dat = nullptr; memset(v.x_sep, 0, sizeof v.x_sep);
 }
 
-static int emit(b200_engine *e, const std::string &s, char *out, size_t cap, size_t *out_len)
+static int emit(b200_engine *e, const std::string &s, uint64_t bound, char *out, size_t cap, size_t *out_len)
 {
+    if (s.size() > bound) { e->err = "internal: output " + std::to_string(s.size()) + " exceeds bound " + std::to_string(bound); return -1; }
     *out_len = s.size();
     if (out) { if (s.size() > cap) { e->err = "output buffer too small"; return -2; } memcpy(out, s.data(), s.size()); }
     return 0;
@@ -268,9 +268,8 @@ int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c, char *out,
         uint32_t len = mp_line_size(v, cf, col >> 5, col, s0);
         if (use_ent) {   // the sums the device derives the line length from must reproduce mp_line_size
             cov += diff[(size_t)col];
-            MpFileSz s1; s1.nplp = cov; s1.cnt = cov - (int32_t)fail[(size_t)col]; s1.seq_len = (uint32_t)s1.cnt + extra[(size_t)col]; s1.bp_len = 0; s1.bp5_len = 0;
-            uint32_t len1 = 0;
-            if ((s1.nplp > 0 || (cf.all && col < v.ncols_all)) && bed_pass(v, col)) len1 = mp_head_len(v, col) + mp_file_section_len(cf, s1) + 1;
+            MpFileSz s1;
+            const uint32_t len1 = mp_sums_line_size(v, cf, col, cov, fail[(size_t)col], extra[(size_t)col], &s1);
             if (len1 != len || (len && (s1.nplp != s0.nplp || s1.cnt != s0.cnt || s1.seq_len != s0.seq_len))) {
                 e->err = "emulation harness: order-free line size differs from mp_line_size at column " + std::to_string(col); return -1;
             }
@@ -281,35 +280,24 @@ int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c, char *out,
         if (use_ent) mp_line_write_ent(v, cf, col, s0, &s[at], E.data(), E2.data());
         else mp_line_write(v, cf, col >> 5, col, s0, &s[at]);
     }
-    return emit(e, s, out, cap, out_len);
+    return emit(e, s, mpileup_text_bound(totals(e, e->ncols_max), *c), out, cap, out_len);
 }
 
-uint64_t b200_mpileup_text_bound(const b200_engine_t *e, const b200_mpileup_conf_t *c)
-{
-    size_t n = 0;
-    return b200_mpileup_text(const_cast<b200_engine_t *>(e), c, nullptr, 0, &n) == 0 ? n + 64 : 0;
-}
-int b200_depth_text(b200_engine_t *e, const b200_depth_conf_t *c, char *out, size_t cap, size_t *out_len);
-uint64_t b200_depth_text_bound(const b200_engine_t *e)
-{
-    // every row: name, tab, position, (tab, depth) per file, newline
-    return (uint64_t)e->ncols_max * (e->name.size() + 1 + 20 + (uint64_t)e->b.n_files * 12 + 1) + 64;
-}
+uint64_t b200_mpileup_text_bound(const b200_engine_t *e, const b200_mpileup_conf_t *c) { return mpileup_text_bound(totals(e, e->ncols_max), *c); }
+uint64_t b200_depth_text_bound(const b200_engine_t *e) { return depth_text_bound(totals(e, e->ncols_max)); }
 int b200_depth_text(b200_engine_t *e, const b200_depth_conf_t *c, char *out, size_t cap, size_t *out_len)
 {
     View v; fill_view(e, v, c->bed_beg, c->bed_end, c->n_bed, c->bed_active, c->all);
     DpConf cf{c->min_qual, c->count_del, c->all};
     std::string s;
     for (int32_t col = 0; col < v.ncols; ++col) {
-        bool any = false; std::vector<int32_t> d((size_t)v.n_files);
-        for (int f = 0; f < v.n_files; ++f) { DpCol o; dp_file_column(v, cf, f, col >> 5, col, o); d[(size_t)f] = o.depth; any |= o.spanned; }
-        if (!any && !(cf.all && col < v.ncols_all)) continue;
-        if (!bed_pass(v, col)) continue;
-        s += e->name; s += '\t'; s += std::to_string(v.win_base + col + 1);
-        for (int f = 0; f < v.n_files; ++f) { s += '\t'; s += std::to_string(d[(size_t)f]); }
-        s += '\n';
+        int32_t d0 = 0;
+        const uint32_t len = dp_line_size(v, cf, col >> 5, col, d0);
+        if (!len) continue;
+        const size_t at = s.size(); s.resize(at + len, '?');
+        dp_line_write(v, cf, col >> 5, col, d0, &s[at]);
     }
-    return emit(e, s, out, cap, out_len);
+    return emit(e, s, depth_text_bound(totals(e, v.ncols)), out, cap, out_len);
 }
 
 int b200_coverage(b200_engine_t *e, const b200_coverage_conf_t *c, b200_coverage_sums_t *sums)
@@ -317,9 +305,9 @@ int b200_coverage(b200_engine_t *e, const b200_coverage_conf_t *c, b200_coverage
     View v; fill_view(e, v, nullptr, nullptr, 0, 0, 0);
     memset(sums, 0, sizeof *sums);
     for (int32_t col = 0; col < v.ncols; ++col) {
-        CvCol o; cv_column(v, c->min_baseQ, col >> 5, col, o);
-        sums->missing_qual += o.missing;
-        if (o.count_base && o.depth >= (uint32_t)c->min_depth) { sums->n_covered_bases++; sums->summed_coverage += o.depth; sums->summed_baseQ += o.sum_bq; sums->quality_bases += o.qbases; }
+        unsigned long long a[5] = {0, 0, 0, 0, 0};
+        cv_sums(v, c->min_baseQ, c->min_depth, col, a);
+        sums->n_covered_bases += a[0]; sums->summed_coverage += a[1]; sums->summed_baseQ += a[2]; sums->quality_bases += a[3]; sums->missing_qual += a[4];
     }
     return 0;
 }
@@ -327,8 +315,7 @@ int b200_coverage_hist(b200_engine_t *e, const b200_coverage_conf_t *c, int64_t 
 {
     View v; fill_view(e, v, nullptr, nullptr, 0, 0, 0);
     for (int32_t col = 0; col < v.ncols; ++col) {
-        CvCol o; cv_column(v, c->min_baseQ, col >> 5, col, o);
-        const uint32_t add = plot_depth ? o.depth : ((o.count_base && o.depth >= (uint32_t)c->min_depth) ? 1u : 0u);
+        const uint32_t add = cv_hist_add(v, c->min_baseQ, c->min_depth, plot_depth, col);
         const int64_t bin = ((int64_t)col - (beg - v.win_base)) / bin_width;
         if (add && bin >= 0 && bin < n_bins) hist[bin] += add;
     }
@@ -337,22 +324,14 @@ int b200_coverage_hist(b200_engine_t *e, const b200_coverage_conf_t *c, int64_t 
 int b200_bedcov(b200_engine_t *e, int32_t skip_dn, int32_t min_depth, uint64_t *cnt, uint64_t *pcov)
 {
     View v; fill_view(e, v, nullptr, nullptr, 0, 0, 0);
-    const bool dn = skip_dn || min_depth >= 0;
     for (int f = 0; f < v.n_files; ++f) { cnt[f] = 0; if (pcov) pcov[f] = 0; }
     for (int32_t c = 0; c < v.ncols; ++c) {
-        std::vector<int32_t> pd((size_t)v.n_files, 0); bool any = false;
+        if (!bc_column_live(v, c >> 5, c)) continue;
         for (int f = 0; f < v.n_files; ++f) {
-            const ReadRange rr = read_range(v, f, c >> 5);
-            for (int32_t t_ = 0; t_ < rr.n; ++t_) {
-                const int32_t i = range_at(rr, t_);
-                const ReadDesc d = v.desc[i];
-                if (c < d.rpos || c >= d.rend) continue;
-                any = true; ++pd[(size_t)f];
-                if (dn) { Ent en; resolve(v, d, c, en); if (en.is_del || en.is_refskip) --pd[(size_t)f]; }
-            }
+            unsigned long long pd, ge;
+            bc_file_column(v, skip_dn, min_depth, f, c >> 5, c, pd, ge);
+            cnt[f] += pd; if (pcov) pcov[f] += ge;
         }
-        if (!any) continue;
-        for (int f = 0; f < v.n_files; ++f) { cnt[f] += (uint64_t)pd[(size_t)f]; if (pcov && min_depth >= 0 && pd[(size_t)f] >= min_depth) pcov[f]++; }
     }
     return 0;
 }
@@ -379,11 +358,8 @@ int b200_pileup_entries(b200_engine_t *e, int32_t file, int64_t beg, int64_t end
             const int32_t i = range_at(rr, t_);
             const ReadDesc d = v.desc[i];
             if (c < d.rpos || c >= d.rend) continue;
-            Ent en; resolve(v, d, c, en);
-            if (en.k < 0) { const uint32_t *cg = v.cigar + d.cig_off; int k = 0; while (!is_mop(cg[k] & 0xf)) ++k; en.k = k; }
             b200_pileup1_t p; memset(&p, 0, sizeof p);
-            p.read = i; p.qpos = en.qpos; p.indel = en.indel; p.cigar_ind = en.k;
-            p.is_del = en.is_del; p.is_head = en.is_head; p.is_tail = en.is_tail; p.is_refskip = en.is_refskip;
+            pileup1_of(v, d, i, c, p);
             all.push_back(p); ++n;
         }
         col_n[c64 - rb] = n;
