@@ -1,5 +1,6 @@
 // cli.cpp -- `b200samtools mpileup|depth|coverage|bedcov|gl`: the reference's CLI surface
-// for the pileup hot path, driving the CUDA engine through its C ABI.
+// for the pileup hot path, driving the CUDA engine through its C ABI; `index` writes the
+// BAI / CSI those commands read a region through.
 //
 // Option surfaces follow bam_plcmd.c:1096-1223 (mpileup), bam2depth.c:757-882
 // (depth) and coverage.c:343-424 (coverage), SURVEY.md Appendix B.  What stays
@@ -47,11 +48,14 @@ struct FileData {
     int64_t n_no_tid = 0;
 };
 
+// With a region, a BAM input is read through its index (idx_fn, or the one found next to it) when there is one: only the
+// blocks that hold the region's records are inflated.  Without an index the reader scans the file.
 bool load_file(const std::string &fn, const std::string &fai, const char *reg, FileData &fd, int &rtid, int64_t &rbeg, int64_t &rend,
-               const char *cmd)
+               const char *cmd, const std::string &idx_fn = "")
 {
     fd.rd = AlnReader::open(fn, fai);
     if (!fd.rd) { fprintf(stderr, "[%s] failed to open %s: %s\n", cmd, fn.c_str(), strerror(errno)); return false; }
+    if (reg && !fd.rd->open_index(idx_fn)) { fprintf(stderr, "[%s] %s\n", cmd, fd.rd->error().c_str()); return false; }
     if (reg && !fd.rd->set_region(reg, rtid, rbeg, rend)) {
         fprintf(stderr, "[E::%s] fail to parse region '%s' with %s\n", cmd, reg, fn.c_str());
         return false;
@@ -359,7 +363,7 @@ uint8_t mp_host_bits(const MpOpts &o, const Header &h, Record &r, bool has_ref)
     return rb;
 }
 
-int run_mpileup(MpOpts &o, const std::vector<std::string> &fn)
+int run_mpileup(MpOpts &o, const std::vector<std::string> &fn, const std::vector<std::string> &idx_fn)
 {
     const int nfn = (int)fn.size();
     if (nfn == 0) { fprintf(stderr, "[mpileup] no input file/data given\n"); return 1; }
@@ -368,7 +372,7 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn)
     const std::string fai = o.fa_fn ? std::string(o.fa_fn) + ".fai" : "";
     for (int i = 0; i < nfn; ++i) {
         int t = 0; int64_t b = 0, e = POS_MAX;
-        if (!load_file(fn[(size_t)i], fai, o.reg, fd[(size_t)i], t, b, e, "mpileup")) return 1;
+        if (!load_file(fn[(size_t)i], fai, o.reg, fd[(size_t)i], t, b, e, "mpileup", idx_fn.empty() ? "" : idx_fn[(size_t)i])) return 1;
         if (i == 0) { tid0 = t; beg0 = b; end0 = e; }
     }
     const Header &h = fd[0].rd->header();
@@ -634,7 +638,7 @@ int main_mpileup(int argc, char **argv, bool gl)
         if (o.n_xfields && o.out_qpos5) { fprintf(stderr, "b200samtools mpileup: --output-BP-5 together with --output-QNAME/--output-extra fields is not available on the device path\n"); return 1; }
     }
     if (argc == 1) { fprintf(stderr, "\nUsage: samtools mpileup [options] in1.bam [in2.bam [...]]\n"); return 1; }
-    std::vector<std::string> fn;
+    std::vector<std::string> fn, idx_fn;   // -X: the data files, then their index files in the same order
     if (file_list) {
         if (has_index_file) { fprintf(stderr, "Error: The -b option cannot be combined with -X\n"); return 1; }
         if (!read_file_list(file_list, fn)) return 1;
@@ -642,8 +646,9 @@ int main_mpileup(int argc, char **argv, bool gl)
         int n = argc - optind;
         if (has_index_file) { if (n % 2) { fprintf(stderr, "Odd number of filenames detected! Each BAM file should have an index file\n"); return 1; } n /= 2; }
         for (int i = 0; i < n; ++i) fn.push_back(argv[optind + i]);
+        if (has_index_file) for (int i = 0; i < n; ++i) idx_fn.push_back(argv[optind + n + i]);
     }
-    return run_mpileup(o, fn);
+    return run_mpileup(o, fn, idx_fn);
 }
 
 // ----------------------------------------------------------------------------- depth
@@ -651,6 +656,7 @@ int main_depth(int argc, char **argv)
 {
     int flag = F_UNMAP | F_SECONDARY | F_DUP | F_QCFAIL, incl = 0, require = 0, min_qual = 0, min_mqual = 0, min_len = 0;
     int skip_del = 1, header = 0, all_pos = 0, remove_overlaps = 0, tmp;
+    bool has_index_file = false;
     const char *reg = nullptr, *file_list = nullptr, *out_fn = nullptr;
     std::unique_ptr<Bed> bed;
     static const struct option lo[] = { {"min-MQ", 1, 0, 'Q'}, {"min-mq", 1, 0, 'Q'}, {"min-BQ", 1, 0, 'q'}, {"min-bq", 1, 0, 'q'},
@@ -662,7 +668,8 @@ int main_depth(int argc, char **argv)
         case 'a': all_pos++; break;
         case 'b': bed = Bed::load(optarg); if (!bed) { fprintf(stderr, "samtools depth: Could not read file \"%s\"\n", optarg); return 1; } break;
         case 'f': file_list = optarg; break;
-        case 'd': case 'm': case '@': case 'X': break;
+        case 'd': case 'm': case '@': break;
+        case 'X': has_index_file = true; break;
         case 'g': tmp = parse_flag(optarg); if (tmp < 0) { fprintf(stderr, "samtools depth: Unknown flag '%s'\n", optarg); return 1; } flag &= ~tmp; break;
         case 'G': tmp = parse_flag(optarg); if (tmp < 0) { fprintf(stderr, "samtools depth: Unknown flag '%s'\n", optarg); return 1; } flag |= tmp; break;
         case 1: tmp = parse_flag(optarg); if (tmp < 0) { fprintf(stderr, "samtools depth: Unknown flag '%s'\n", optarg); return 1; } incl |= tmp; break;
@@ -678,9 +685,14 @@ int main_depth(int argc, char **argv)
         default: fprintf(stderr, "Usage: samtools depth [options] in.bam [in.bam ...]\n"); return 1;
         }
     }
-    std::vector<std::string> fn;
+    std::vector<std::string> fn, idx_fn;   // -X: the data files, then their index files in the same order
     if (file_list) { if (!read_file_list(file_list, fn)) return 1; }
-    else for (int i = optind; i < argc; ++i) fn.push_back(argv[i]);
+    else {
+        int n = argc - optind;
+        if (has_index_file) { if (n % 2) { fprintf(stderr, "Odd number of filenames detected! Each BAM file should have an index file\n"); return 1; } n /= 2; }
+        for (int i = 0; i < n; ++i) fn.push_back(argv[optind + i]);
+        if (has_index_file) for (int i = 0; i < n; ++i) idx_fn.push_back(argv[optind + n + i]);
+    }
     if (fn.empty()) { fprintf(stderr, "Usage: samtools depth [options] in.bam [in.bam ...]\n"); return 1; }
     const int nfn = (int)fn.size();
     std::vector<FileData> fd((size_t)nfn);
@@ -688,7 +700,7 @@ int main_depth(int argc, char **argv)
     for (int i = 0; i < nfn; ++i) {
         int t = 0; int64_t b = 0, e = POS_MAX;
         fd[(size_t)i].rd = nullptr;
-        if (!load_file(fn[(size_t)i], "", reg, fd[(size_t)i], t, b, e, "depth")) return 1;
+        if (!load_file(fn[(size_t)i], "", reg, fd[(size_t)i], t, b, e, "depth", idx_fn.empty() ? "" : idx_fn[(size_t)i])) return 1;
         if (i == 0) { tid0 = t; beg0 = b; end0 = e; }
     }
     const Header &h = fd[0].rd->header();
@@ -998,18 +1010,20 @@ int main_coverage(int argc, char **argv)
 // `samtools bedcov` (bedcov.c): for every BED line the reference opens an index query over [beg,end) and runs the
 // multi-file pileup iterator with the column reducers of bedcov.c:316-331.  Here every line stages the records that
 // overlap its interval (B200_MODE_COVERAGE read filters: the -g/-G flag set and -Q) and b200_bedcov() reduces the window
-// on the device.  BED lines may name the reference sequences in any order, so the inputs are decoded completely up front
-// (the reference has random access through the BAI; this driver has no index reader).
+// on the device.  When every input has an index (found next to it, or named by -X), each line queries it like the
+// reference does and only the line's records are decoded.  Otherwise BED lines may name the reference sequences in any
+// order, so the inputs are decoded completely up front.
 int main_bedcov(int argc, char **argv)
 {
     int c, min_mapQ = 0, skip_DN = 0, do_rcount = 0, min_depth = -1, max_depth = INT_MAX, print_header = 0, hdr = 0, status = 0, tflags;
+    bool has_index_file = false;
     int flags = F_UNMAP | F_SECONDARY | F_QCFAIL | F_DUP;
     static const struct option lo[] = { {"min-MQ", 1, 0, 'Q'}, {"min-mq", 1, 0, 'Q'}, {"max-depth", 1, 0, 1000}, {0, 0, 0, 0} };
     optind = 1;
     while ((c = getopt_long(argc, argv, "Q:Xg:G:jd:Hc", lo, nullptr)) >= 0) {
         switch (c) {
         case 'Q': min_mapQ = atoi(optarg); break;
-        case 'X': break;
+        case 'X': has_index_file = true; break;
         case 'c': do_rcount = 1; break;
         case 'H': print_header = 1; break;
         case 'g': tflags = parse_flag(optarg); if (tflags < 0 || tflags > 4095) { fprintf(stderr, "[bedcov] Flag value \"%s\" is not supported\n", optarg); return 1; } flags &= ~tflags; break;
@@ -1021,15 +1035,26 @@ int main_bedcov(int argc, char **argv)
         }
     }
     if (optind + 2 > argc) { fprintf(stderr, "Usage: samtools bedcov [options] <in.bed> <in1.bam> [...]\n"); return 1; }
-    const int n = argc - optind - 1;
+    int n = argc - optind - 1;
+    if (has_index_file) {   // -X: the data files, then their index files in the same order
+        if (n % 2) { fprintf(stderr, "Odd number of filenames detected! Each BAM file should have an index file\n"); return 1; }
+        n /= 2;
+    }
     char **fn = argv + optind + 1;
     if (!print_header) hdr = 1;
     std::vector<FileData> fd((size_t)n);
+    bool indexed = true;
     for (int i = 0; i < n; ++i) {
         int t = 0; int64_t b = 0, e = POS_MAX;
         if (!load_file(fn[i], "", nullptr, fd[(size_t)i], t, b, e, "bedcov")) { fprintf(stderr, "ERROR: fail to open index BAM file '%s'\n", fn[i]); return 2; }
-        fd[(size_t)i].keep_all = true;
-        for (int tid = 0; tid < fd[(size_t)i].rd->header().n_ref(); ++tid) if (!load_tid(fd[(size_t)i], tid, "bedcov")) return 2;
+        if (!fd[(size_t)i].rd->open_index(has_index_file ? fn[n + i] : "")) { fprintf(stderr, "[bedcov] %s\n", fd[(size_t)i].rd->error().c_str()); return 2; }
+        indexed = indexed && fd[(size_t)i].rd->has_index();
+    }
+    if (!indexed) {
+        for (int i = 0; i < n; ++i) {
+            fd[(size_t)i].keep_all = true;
+            for (int tid = 0; tid < fd[(size_t)i].rd->header().n_ref(); ++tid) if (!load_tid(fd[(size_t)i], tid, "bedcov")) return 2;
+        }
     }
     const Header &h = fd[0].rd->header();
     // per file and reference sequence: running maximum of the record ends, so that the first record that can reach an
@@ -1080,6 +1105,15 @@ int main_bedcov(int argc, char **argv)
             pb.clear();
             for (int i = 0; i < n; ++i) {
                 pb.begin_file();
+                if (indexed) {
+                    AlnReader &rd = *fd[(size_t)i].rd;
+                    rd.query(tid, beg, end);
+                    Record r;
+                    int ret;
+                    while ((ret = rd.next(r)) == 0) pb.add(r, 0, false);
+                    if (ret < -1) { fprintf(stderr, "samtools bedcov: error reading from input file %s\n", fn[i]); return 2; }
+                    continue;
+                }
                 if (tid >= (int)fd[(size_t)i].by_tid.size()) continue;
                 const std::vector<Record> &v = fd[(size_t)i].by_tid[(size_t)tid];
                 const std::vector<int64_t> &rm = runmax[(size_t)i][(size_t)tid];
@@ -1111,17 +1145,47 @@ int main_bedcov(int argc, char **argv)
     return status;
 }
 
+// ----------------------------------------------------------------------------- index
+// `samtools index [-b|-c] [-m INT] in.bam [out.index]`: a BAI (default) or a CSI (-c; -m sets its min_shift and implies -c)
+// of a coordinate-sorted BGZF BAM, written next to it unless named.
+int main_index(int argc, char **argv)
+{
+    bool csi = false;
+    int min_shift = 14, c;
+    const char *usage = "Usage: b200samtools index [-b|-c] [-m INT] <in.bam> [out.index]\n";
+    optind = 1;
+    while ((c = getopt(argc, argv, "bcm:")) >= 0) {
+        switch (c) {
+        case 'b': csi = false; break;
+        case 'c': csi = true; break;
+        case 'm': {
+            char *e; const long v = strtol(optarg, &e, 10);
+            if (*e || v < 1 || v > 30) { fprintf(stderr, "[bam_index] -m takes a min_shift from 1 to 30\n"); return 1; }
+            min_shift = (int)v; csi = true;
+            break;
+        }
+        default: fputs(usage, stderr); return 1;
+        }
+    }
+    if (argc - optind < 1 || argc - optind > 2) { fputs(usage, stderr); return 1; }
+    const std::string in = argv[optind], out = argc - optind == 2 ? argv[optind + 1] : in + (csi ? ".csi" : ".bai");
+    std::string err;
+    if (build_index(in, out, csi, min_shift, err) != 0) { fprintf(stderr, "[bam_index] %s\n", err.c_str()); return 1; }
+    return 0;
+}
+
 }  // namespace
 
 int main(int argc, char **argv)
 {
-    if (argc < 2) { fprintf(stderr, "Usage: b200samtools <mpileup|depth|coverage|bedcov|gl> [options]\n"); return 1; }
+    if (argc < 2) { fprintf(stderr, "Usage: b200samtools <mpileup|depth|coverage|bedcov|gl|index> [options]\n"); return 1; }
     std::string cmd = argv[1];
     if (cmd == "mpileup") return main_mpileup(argc - 1, argv + 1, false);
     if (cmd == "gl") return main_mpileup(argc - 1, argv + 1, true);
     if (cmd == "depth") return main_depth(argc - 1, argv + 1);
     if (cmd == "coverage") return main_coverage(argc - 1, argv + 1);
     if (cmd == "bedcov") return main_bedcov(argc - 1, argv + 1);
+    if (cmd == "index") return main_index(argc - 1, argv + 1);
     fprintf(stderr, "b200samtools: unrecognized command '%s'\n", argv[1]);
     return 1;
 }
