@@ -256,7 +256,9 @@ int64_t b200_launch_count(const b200_engine_t *e);   /* kernels launched by this
 /* hts_drand48 draws consumed so far by b200_glf (errmod_cal shuffles a column's bases when it holds more than 255; the
  * reference draws from ONE process-wide stream, so a region shard continues from its predecessor's count) */
 uint64_t b200_gl_rng_draws(const b200_engine_t *e);
-/* last b200_mpileup_text(): device time of its three launches -- sizing kernel, tile-offset scan, write kernel */
+/* last b200_mpileup_text(): device time of its three parts.  Default path (one input file, no -O columns): entry pass
+ * (k_mp_entries), line sizes + tile offsets (k_mp_place), gather (k_mp_gather).  General path: sizing kernel, tile-offset
+ * scan, write kernel. */
 void b200_last_mpileup_parts_ms(const b200_engine_t *e, double *ms3);
 
 #ifdef __cplusplus

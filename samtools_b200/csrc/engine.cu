@@ -13,9 +13,11 @@
 // Column stage for text (mpileup, depth): sizes -> offsets -> bytes, no inter-CTA waiting.
 //   (1) sizes.  mpileup, one input file (the default path, mpileup_ent.cuh / mpileup_ss.cuh): a READ-major entry pass formats
 //       every read into 16-bit entries (eight bases per lane, SIMD within a register) and feeds order-free line-length sums
-//       (coverage difference array, failing bases, extra bytes); a scan + a per-column kernel turn them into line lengths.
+//       (coverage difference array, failing bases, extra bytes).
 //       General mpileup path (several files, -O, host string columns) and depth: thread per column.
-//   (2) a single-pass scan of 128-column tile totals gives every tile its byte offset;
+//   (2) offsets.  Default mpileup: one single-pass kernel (k_mp_place) scans the sums into n_plp, sizes every line and gives
+//       every 128-column tile its byte offset; only n_plp and the tile offsets reach HBM.  Other paths: a single-pass scan of
+//       the 128-column tile totals;
 //   (3) bytes.  Default mpileup: the gather -- a warp per 32-column group fetches the entry strings with wide loads (lanes along
 //       the reads), parks them in shared-memory rows and appends them to the lines (lanes along the columns).  Other paths:
 //       one thread per reference position formats its line.  Either way a tile's text is laid out in shared memory with the
@@ -993,22 +995,17 @@ extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c,
     *out_len = 0; e->last_kernel_ms = 0;
     if (nt == 0) return 0;
     ENSURE(out, (size_t)bound + 64);
-    ENSURE(col_n, (size_t)nt * TILE + 1);
-    ENSURE(col_state, ((size_t)nt * TILE * sizeof(MpFileSz) + 7) / 8 + 1);
-    ENSURE(tile_total, (size_t)nt + 1); ENSURE(col_off, (size_t)nt + 2);
+    ENSURE(col_off, (size_t)nt + 2);
     ENSURE(ent, e->qual_bytes + 64 + ENT_PAD); ENSURE(ent2, (size_t)e->sum_rlen_gen + 64 + ENT_PAD);   // front pad + slack for the gather's 80-byte fetches
-    const int nb = nblk(nt, 256);
-    ENSURE(status, (size_t)nb + 1);
-    CK(cudaMemsetAsync(e->status, 0, ((size_t)nb + 1) * 8, e->stream));
-    CK(cudaMemsetAsync(e->d_misc, 0, 8, e->stream));
-    ENSURE(ss_diff, (size_t)ncols + 2); ENSURE(ss_nplp, (size_t)ncols + 2); ENSURE(ss_fail, (size_t)ncols + 1); ENSURE(ss_extra, (size_t)ncols + 1);
+    ENSURE(ss_diff, (size_t)ncols + 3); ENSURE(ss_nplp, (size_t)ncols + 2); ENSURE(ss_fail, (size_t)ncols + 3); ENSURE(ss_extra, (size_t)ncols + 3);   // k_mp_place reads up to ncols + 2
     CK(cudaMemsetAsync(e->ss_diff, 0, ((size_t)ncols + 2) * 4, e->stream));
     CK(cudaMemsetAsync(e->ss_fail, 0, ((size_t)ncols + 1) * 4, e->stream));
     CK(cudaMemsetAsync(e->ss_extra, 0, ((size_t)ncols + 1) * 4, e->stream));
-    const int nbs = nblk((int64_t)ncols + 1, 1024);
-    ENSURE(status2, (size_t)nbs + 1);
-    CK(cudaMemsetAsync(e->status2, 0, ((size_t)nbs + 1) * 8, e->stream));
-    CK(cudaMemsetAsync(e->d_misc + 2, 0, 16, e->stream));      // scan ticket, cursor of the second entry array
+    const int nbp = nblk(ncols, PLACE_COLS);                // k_mp_place blocks; look-back status: coverage (status2), bytes (status)
+    ENSURE(status, (size_t)nbp + 1); ENSURE(status2, (size_t)nbp + 1);
+    CK(cudaMemsetAsync(e->status, 0, ((size_t)nbp + 1) * 8, e->stream));
+    CK(cudaMemsetAsync(e->status2, 0, ((size_t)nbp + 1) * 8, e->stream));
+    CK(cudaMemsetAsync(e->d_misc + 2, 0, 16, e->stream));      // k_mp_place ticket, cursor of the second entry array
     CK(cudaEventRecord(e->ev0, e->stream));
     {
         // one warp per 32 reads, 8 warps per block; up to 64 blocks per SM, so that an 8 Mb window at 30x (1.6 M reads) runs in
@@ -1018,11 +1015,10 @@ extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c,
         if (e->has_ref) k_mp_entries<true><<<rb, 256, 0, e->stream>>>(fmt.v, fmt.cf, e->n, e->ref_codes, e->ss_diff, e->ss_fail, e->ss_extra, e->ent + ENT_PAD, e->ent2 + ENT_PAD, e->d_misc + 3, e->desc);
         else k_mp_entries<false><<<rb, 256, 0, e->stream>>>(fmt.v, fmt.cf, e->n, nullptr, e->ss_diff, e->ss_fail, e->ss_extra, e->ent + ENT_PAD, e->ent2 + ENT_PAD, e->d_misc + 3, e->desc);
         e->launches++;
-        k_ss_scan<<<nbs, 256, 0, e->stream>>>(e->ss_diff, e->ss_nplp, ncols + 1, e->status2, (uint32_t *)(e->d_misc + 2)); e->launches++;
-        k_ss_cols<<<nt, TILE, 0, e->stream>>>(fmt.v, fmt.cf, e->ss_nplp, e->ss_fail, e->ss_extra, e->col_n, (MpFileSz *)e->col_state, e->tile_total); e->launches++;
     }
     CK(cudaEventRecord(e->evA, e->stream));
-    k_scan_u32_to_u64<<<nb, 256, 0, e->stream>>>(e->tile_total, e->col_off, nt, e->status, (uint32_t *)e->d_misc); e->launches++;
+    k_mp_place<<<nbp, 256, 0, e->stream>>>(fmt.v, fmt.cf, e->ss_diff, e->ss_fail, e->ss_extra, e->ss_nplp, e->col_off, nt, e->status2, e->status,
+                                            (uint32_t *)(e->d_misc + 2)); e->launches++;
     CK(cudaEventRecord(e->evB, e->stream));
     {
         MpEntFmt gf; gf.v = fmt.v; gf.cf = fmt.cf; gf.E = e->ent + ENT_PAD; gf.E2 = e->ent2 + ENT_PAD;
@@ -1039,8 +1035,8 @@ extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c,
             const uint64_t want = std::max<uint64_t>(12 * 1024, (avg_tile * 9 / 8 + 1023) & ~1023ull);
             if (want < cap) cap = (uint32_t)want;
         }
-        if (c->out_mapq) k_mp_gather<7, true><<<nt, TILE, cap + 16, e->stream>>>(gf, dg, e->col_n, (const MpFileSz *)e->col_state, e->col_off, e->out, cap, e->use_tma);
-        else k_mp_gather<7, false><<<nt, TILE, cap + 16, e->stream>>>(gf, dg, e->col_n, (const MpFileSz *)e->col_state, e->col_off, e->out, cap, e->use_tma);
+        if (c->out_mapq) k_mp_gather<7, true><<<nt, TILE, cap + 16, e->stream>>>(gf, dg, e->ss_nplp, e->ss_fail, e->ss_extra, e->col_off, e->out, cap, e->use_tma);
+        else k_mp_gather<7, false><<<nt, TILE, cap + 16, e->stream>>>(gf, dg, e->ss_nplp, e->ss_fail, e->ss_extra, e->col_off, e->out, cap, e->use_tma);
         e->launches++;
     }
     CK(cudaEventRecord(e->ev1, e->stream));
@@ -1049,9 +1045,9 @@ extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c,
     CK(cudaStreamSynchronize(e->stream));
     CK(cudaGetLastError());
     float ms = 0; cudaEventElapsedTime(&ms, e->ev0, e->ev1); e->last_kernel_ms = ms;
-    cudaEventElapsedTime(&ms, e->ev0, e->evA); e->last_parts_ms[0] = ms;      // entry strings + sizes
-    cudaEventElapsedTime(&ms, e->evA, e->evB); e->last_parts_ms[1] = ms;      // tile-offset scan
-    cudaEventElapsedTime(&ms, e->evB, e->ev1); e->last_parts_ms[2] = ms;      // gather
+    cudaEventElapsedTime(&ms, e->ev0, e->evA); e->last_parts_ms[0] = ms;      // k_mp_entries: entry strings + line-length sums
+    cudaEventElapsedTime(&ms, e->evA, e->evB); e->last_parts_ms[1] = ms;      // k_mp_place: n_plp, line lengths, tile offsets
+    cudaEventElapsedTime(&ms, e->evB, e->ev1); e->last_parts_ms[2] = ms;      // k_mp_gather
     if (total > bound) { snprintf(e->err, sizeof e->err, "internal: output %llu exceeds bound %llu", total, (unsigned long long)bound); return -1; }
     *out_len = (size_t)total; e->last_out_len = (size_t)total;
     if (out) {

@@ -13,9 +13,10 @@
 //                 the generic cursor into slices of a second array, the warp taking them one by one; their slices come
 //                 from one cursor atomic per warp.  The same pass feeds the line-length sums of mpileup_ss.cuh (coverage
 //                 difference array, failing bases and extra bytes per column): it IS the size pass.
-//   k_mp_gather   COLUMN-MAJOR, one thread per reference position: walks the reads of its 32-column slice in file
-//                 order and appends the non-empty entries to its line (2 bytes per entry, no decoding, no CIGAR walk);
-//                 the tile leaves through the TMA bulk store of text_write_tile.
+//   k_mp_gather   COLUMN-MAJOR, one thread per reference position: derives its line's length and layout from the column's
+//                 sums, walks the reads of its 32-column slice in file order and appends the non-empty entries to its line
+//                 (2 bytes per entry, no decoding, no CIGAR walk); the tile leaves through TMA bulk stores at the offset
+//                 k_mp_place (mpileup_ss.cuh) gave it.
 // Replaces the per-(read, column) formatting loop of the round-1 write kernel (~100 instructions per pair).
 #pragma once
 
@@ -238,8 +239,8 @@ struct MpEntFmt {
 constexpr int ENT_PAD = 64;
 
 // ---- the gather: one warp per 32-column group ------------------------------------------------------------------------
-// The kernel issues every tile-level load (column lengths and states, the tile's output offset, the warp's read range) at
-// entry, before the block scan, so that they cost one round trip together.  Then two phases per round of 32 slice positions
+// The kernel issues every tile-level load (the column's n_plp / fail / extra sums, the tile's output offset, the warp's read
+// range) at entry, before the block scan, so that they cost one round trip together.  Then two phases per round of 32 slice positions
 // of the group's read range, with shared memory as the transpose buffer:
 //   fetch   LANES ALONG THE READS: each lane loads its read's whole 32-byte descriptor (one sector: the second-array offset
 //           of a read with indels does not wait on its flags).  Reads that reach the group get a row (ballot compaction, file
@@ -365,8 +366,8 @@ __device__ __forceinline__ void gather_group(const MpEntFmt &fmt, const MpEntFmt
 }
 
 template <int MIN_CTAS, bool OUT_MAPQ>
-__global__ void __launch_bounds__(TILE, MIN_CTAS) k_mp_gather(MpEntFmt fmt, const MpEntFmt *gfmt, const uint32_t *len_in, const MpFileSz *st_in, const uint64_t *tile_base,
-                                                              char *out, uint32_t smem_cap, int use_tma)
+__global__ void __launch_bounds__(TILE, MIN_CTAS) k_mp_gather(MpEntFmt fmt, const MpEntFmt *gfmt, const int32_t *nplp, const uint32_t *fail, const uint32_t *extra,
+                                                              const uint64_t *tile_base, char *out, uint32_t smem_cap, int use_tma)
 {
     extern __shared__ __align__(16) char s_text[];
     __shared__ uint32_t s_ws[TILE / 32];
@@ -375,14 +376,15 @@ __global__ void __launch_bounds__(TILE, MIN_CTAS) k_mp_gather(MpEntFmt fmt, cons
     const int32_t ncols = fmt.v.ncols;
     const int32_t c = (int32_t)blockIdx.x * TILE + (int32_t)threadIdx.x;
     const int32_t c0 = (int32_t)(blockIdx.x * TILE + (threadIdx.x & ~31u));
-    // Every tile-level load goes out here, unconditionally and before the block scan, so that they share one round trip:
-    // the column's length and state (both arrays cover the whole last tile; beyond ncols the length is not written and
-    // is replaced by 0), the tile's output offset, and the warp's read range (a warp past the window reads the last group's).
-    uint32_t len = len_in[c];
-    const MpFileSz stt = st_in[c];
-    if (c >= ncols) len = 0;
+    // Every tile-level load goes out here, before the block scan, so that they share one round trip: the column's sums
+    // (k_mp_place, k_mp_entries), the tile's output offset, and the warp's read range (a warp past the window reads the
+    // last group's).  The line's length and state follow from the sums as in k_mp_place.
+    int32_t np = 0; uint32_t nf = 0, nx = 0;
+    if (c < ncols) { np = nplp[c]; nf = fail[c]; nx = extra[c]; }
     const uint64_t base = tile_base[blockIdx.x];
     const ReadRange rr = read_range(fmt.v, 0, min(c0 >> 5, fmt.v.n_tiles - 1));   // the same for the 32 lanes
+    MpFileSz stt;
+    const uint32_t len = c < ncols ? mp_sums_line_size(fmt.v, fmt.cf, c, np, nf, nx, &stt) : 0u;
     uint32_t total;
     const uint32_t off = block_excl_scan<TILE>(len, s_ws, total);
     if (total == 0) return;
