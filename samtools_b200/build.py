@@ -2,6 +2,7 @@
 
   samtools_b200/lib/libb200pileup.so   CUDA engine + C ABI (include/b200_pileup.h)
   samtools_b200/bin/b200samtools       host CLI (C++), linked against the engine
+  tests/*/_build/*                     test clients (compat tier, scan check)
   oracle/_build/*                      CPU oracle (test infrastructure, built by its own Makefile)
 
 Everything is built in-tree, so the package runs from the source tree without an install step.
@@ -82,6 +83,17 @@ def build_read_ops_client(force=False):
     return exe
 
 
+def build_scan_check(force=False):
+    """tests/gpu/scan_check: runs the engine's single-pass scans (csrc/scan.cuh) on inputs the GPU test writes."""
+    src = os.path.join(ROOT, 'tests', 'gpu', 'scan_check.cu')
+    exe = os.path.join(ROOT, 'tests', 'gpu', '_build', 'scan_check')
+    if force or _newer(exe, [src, os.path.join(CSRC, 'scan.cuh')]):
+        os.makedirs(os.path.dirname(exe), exist_ok=True)
+        nvcc = shutil.which('nvcc') or '/usr/local/cuda/bin/nvcc'
+        subprocess.run([nvcc, '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-std=c++17', '-o', exe, src], check=True)
+    return exe
+
+
 def build_oracle():
     subprocess.run(['make', '-s', '-C', os.path.join(ROOT, 'oracle')], check=True)
     subprocess.run(['make', '-s', '-C', os.path.join(ROOT, 'oracle'), 'ref'], check=True)
@@ -92,6 +104,7 @@ def build_all(force=False, verbose=False):
     build_engine(force, verbose)
     build_cli(force)
     build_compat_client(force)
+    build_scan_check(force)
     build_oracle()
     build_read_ops_client(force)
 

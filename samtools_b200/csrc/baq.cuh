@@ -472,10 +472,10 @@ int launch_baq(b200_engine *e, const RawSoA &r, const b200_stage_conf_t &cf)
     BaqPlan *plan = (BaqPlan *)(e->baq_idx + 2 * nr);
     // band-7 reads run on the register kernel (k_baq_reg), everything else (wide bands, very long reads) on the warp kernel;
     // B200_BAQ_REG=0 (read per handle when it is created) sends every read to the warp kernel (cross-check)
-    CK(cudaMemsetAsync(e->d_misc + 16, 0, 16 * 8, e->stream));
-    k_baq_plan<<<nblk(n, 256), 256, 0, e->stream>>>(r, cf, e->state, plan, idx, idx2, e->baq_reg, e->d_misc + 16); e->launches++;
+    CK(cudaMemsetAsync(e->d_misc + MISC_BAQ, 0, 16 * 8, e->stream));
+    k_baq_plan<<<nblk(n, 256), 256, 0, e->stream>>>(r, cf, e->state, plan, idx, idx2, e->baq_reg, e->d_misc + MISC_BAQ); e->launches++;
     unsigned long long h[5];
-    CK(cudaMemcpyAsync(h, e->d_misc + 16, sizeof h, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(h, e->d_misc + MISC_BAQ, sizeof h, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     CK(cudaGetLastError());
     const int64_t n_idx = (int64_t)h[0], n_idx2 = (int64_t)h[3];
@@ -507,7 +507,7 @@ int launch_baq(b200_engine *e, const RawSoA &r, const b200_stage_conf_t &cf)
         warps = (int64_t)blocks * 4;
         if (n_idx2 > 0) CK(cudaStreamSynchronize(e->stream));   // the slab buffer is shared by the two kernels
         if (ensure(e, e->baq_f, e->cap_baq_f, (size_t)warps * slab)) return -1;
-        k_baq<<<blocks, 128, 0, e->stream>>>(r, plan, idx, n_idx, e->baq_f, slab, e->d_q2p, e->d_qthr, e->d_misc + 19 + 8, cf.baq != 3); e->launches++;
+        k_baq<<<blocks, 128, 0, e->stream>>>(r, plan, idx, n_idx, e->baq_f, slab, e->d_q2p, e->d_qthr, e->d_misc + MISC_BAQ + 11, cf.baq != 3); e->launches++;
     }
     CK(cudaGetLastError());
     return 0;

@@ -17,11 +17,14 @@
 //       General mpileup path (several files, -O, host string columns) and depth: thread per column.
 //   (2) offsets.  Default mpileup: one single-pass kernel (k_mp_place) scans the sums into n_plp, sizes every line and gives
 //       every 128-column tile its byte offset; only n_plp and the tile offsets reach HBM.  Other paths: a single-pass scan of
-//       the 128-column tile totals;
+//       the 128-column tile totals.  Every scan here (also the read stage's prefix max of read ends and the offsets of the
+//       max-depth gate, the far-reaching lists, the entry and GL columns) is k_scan or the look-back of scan.cuh, launched
+//       through launch_scan / lookback_state;
 //   (3) bytes.  Default mpileup: the gather -- a warp per 32-column group fetches the entry strings with wide loads (lanes along
 //       the reads), parks them in shared-memory rows and appends them to the lines (lanes along the columns).  Other paths:
 //       one thread per reference position formats its line.  Either way a tile's text is laid out in shared memory with the
-//       destination's 16-byte phase and leaves the SM through cp.async.bulk (TMA) shared->global stores plus <16 B edges.
+//       destination's 16-byte phase and leaves the SM through cp.async.bulk (TMA) shared->global stores plus <16 B edges
+//       (store_staged).
 // HBM traffic per column is ~ the algorithmic bytes (+ the entry strings, written and read once).
 // No tensor cores: integer/byte work.
 #include <cuda_runtime.h>
@@ -42,83 +45,7 @@ using namespace plp;
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { \
     snprintf(e->err, sizeof e->err, "%s:%d %s: %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); return -1; } } while (0)
 
-// ============================== device helpers ===============================
-__device__ __forceinline__ uint64_t ld_acquire_u64(const uint64_t *p)
-{
-    uint64_t v;
-    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_release_u64(uint64_t *p, uint64_t v)
-{
-    asm volatile("st.release.gpu.global.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
-}
-#define ST_FLAG(w) ((w) >> 62)
-#define ST_VAL(w) ((w) & 0x3fffffffffffffffULL)
-
-// status words are self-contained (flag + value in one 64-bit word), so polling
-// needs no acquire: relaxed gpu-scope accesses go to L2 and, unlike ld.acquire,
-// do not invalidate the SM's L1 (CCTL.IVALL) under the feet of the other warps.
-__device__ __forceinline__ uint64_t ld_relaxed_u64(const uint64_t *p)
-{
-    uint64_t v;
-    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_relaxed_u64(uint64_t *p, uint64_t v)
-{
-    asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
-}
-
-// decoupled look-back (sum), executed by ONE FULL WARP: 32 predecessors are
-// inspected per round.  Returns the exclusive prefix of tile `t` (all lanes).
-__device__ uint64_t lookback_sum(uint64_t *st, int t, uint64_t agg)
-{
-    const int lane = threadIdx.x & 31;
-    if (t == 0) { if (lane == 0) st_relaxed_u64(&st[0], (2ULL << 62) | agg); return 0; }
-    if (lane == 0) st_relaxed_u64(&st[t], (1ULL << 62) | agg);
-    uint64_t excl = 0;
-    for (int base = t - 1;; base -= 32) {
-        const int j = base - lane;
-        uint64_t w;
-        unsigned m2, need;
-        for (;;) {
-            w = j >= 0 ? ld_relaxed_u64(&st[j]) : (2ULL << 62);      // before tile 0: inclusive prefix 0
-            m2 = __ballot_sync(0xffffffffu, ST_FLAG(w) == 2);
-            need = m2 ? ((2u << (__ffs(m2) - 1)) - 1u) : 0xffffffffu;  // lanes up to the nearest inclusive prefix
-            if ((__ballot_sync(0xffffffffu, ST_FLAG(w) == 0) & need) == 0) break;
-            __nanosleep(40);
-        }
-        uint64_t x = ((need >> lane) & 1u) ? ST_VAL(w) : 0;
-#pragma unroll
-        for (int o = 16; o; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-        excl += x;
-        if (m2) break;
-    }
-    if (lane == 0) st_relaxed_u64(&st[t], (2ULL << 62) | (excl + agg));
-    return excl;
-}
-
-template <int T>
-__device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t *warp_sums, uint32_t &total)
-{
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    uint32_t x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { uint32_t y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
-    if (lane == 31) warp_sums[w] = x;
-    __syncthreads();
-    if (w == 0) {
-        uint32_t s = lane < T / 32 ? warp_sums[lane] : 0;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { uint32_t y = __shfl_up_sync(0xffffffffu, s, o); if (lane >= o) s += y; }
-        if (lane < T / 32) warp_sums[lane] = s;
-    }
-    __syncthreads();
-    total = warp_sums[T / 32 - 1];
-    uint32_t base = w ? warp_sums[w - 1] : 0;
-    return base + x - v;
-}
+#include "scan.cuh"
 
 // ============================== read stage ===================================
 // (arithmetic in plp_stage.h; one thread per read)
@@ -179,53 +106,6 @@ __global__ void k_build_desc(RawSoA r, b200_stage_conf_t cf, const uint8_t *stat
     merge_acc(loc, acc);
 }
 
-// inclusive prefix max of endv[] (single pass, decoupled look-back, one file at a time)
-__global__ void k_scan_max(const int32_t *in, int32_t *out, int64_t n, uint64_t *st, uint32_t *ticket)
-{
-    constexpr int T = 256, IPT = 8;
-    __shared__ int s_tile;
-    __shared__ int32_t s_w[T / 32];
-    __shared__ int32_t s_excl;
-    if (threadIdx.x == 0) s_tile = (int)atomicAdd(ticket, 1u);
-    __syncthreads();
-    const int t = s_tile;
-    const int64_t base = (int64_t)t * T * IPT + (int64_t)threadIdx.x * IPT;
-    int32_t v[IPT], m = INT32_MIN;
-#pragma unroll
-    for (int j = 0; j < IPT; ++j) { v[j] = base + j < n ? in[base + j] : INT32_MIN; m = max(m, v[j]); v[j] = m; }
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    int32_t x = m;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { int32_t y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x = max(x, y); }
-    if (lane == 31) s_w[w] = x;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int32_t run = INT32_MIN;
-        for (int k = 0; k < T / 32; ++k) { int32_t tmp = s_w[k]; s_w[k] = run; run = max(run, tmp); }
-        // publish aggregate / look back (values biased to unsigned)
-        const uint64_t agg = (uint64_t)((int64_t)run - INT32_MIN);
-        uint64_t excl = 0;
-        if (t == 0) st_relaxed_u64(&st[0], (2ULL << 62) | agg);
-        else {
-            st_relaxed_u64(&st[t], (1ULL << 62) | agg);
-            for (int j = t - 1;; --j) {
-                uint64_t wv;
-                while (ST_FLAG(wv = ld_relaxed_u64(&st[j])) == 0) { __nanosleep(20); }
-                { const uint64_t pv = ST_VAL(wv); if (pv > excl) excl = pv; }
-                if (ST_FLAG(wv) == 2) break;
-            }
-            st_relaxed_u64(&st[t], (2ULL << 62) | (excl > agg ? excl : agg));
-        }
-        s_excl = (int32_t)((int64_t)excl + INT32_MIN);
-    }
-    __syncthreads();
-    int32_t pre = max(s_excl, s_w[w]);
-    int32_t left = __shfl_up_sync(0xffffffffu, x, 1);
-    if (lane > 0) pre = max(pre, left);
-#pragma unroll
-    for (int j = 0; j < IPT; ++j) if (base + j < n) out[base + j] = max(pre, v[j]);
-}
-
 // per 32-column group: the [lo,hi) slice of each file's reads that can cover it (plp_stage.h group_slice)
 __global__ void k_ranges(const ReadDesc *desc, const int32_t *pmax, const int64_t *file_start, int n_files,
                          int32_t n_groups, int32_t *glo, int32_t *ghi, int *max_range)
@@ -278,19 +158,32 @@ __global__ void k_ovf_sort(const int32_t *off, int32_t *idx, int64_t n_lists)   
     int32_t *a = idx + off[k]; const int32_t m = off[k + 1] - off[k];
     for (int32_t i = 1; i < m; ++i) { const int32_t x = a[i]; int32_t j = i - 1; while (j >= 0 && a[j] > x) { a[j + 1] = a[j]; --j; } a[j + 1] = x; }
 }
-__global__ void k_scan_u32_excl_i32(const uint32_t *in, int32_t *out, int32_t n, uint64_t *st, uint32_t *ticket);
 
 // ============================== column stage =================================
 constexpr int TILE = 128;
 
-// shared->global bulk store (TMA engine, SASS UBLKCP); all addresses/sizes 16 B aligned
-__device__ __forceinline__ void bulk_store_s2g(void *gdst, const void *ssrc, uint32_t bytes)
+// Stores the staged text sb[beg, beg + len) to g[beg, beg + len), where sb[0] and g[0] have the same 16-byte phase `phase`:
+// the ragged head (to the next 16-byte boundary) and tail by the lanes, the aligned body through one cp.async.bulk (TMA)
+// shared->global store (SASS UBLKCP).  Called by all NT threads of a group, a warp (NT = 32) or the block (NT = blockDim.x),
+// after they wrote the text.  The order is the one the CUDA programming guide gives for TMA stores: every writer makes
+// its shared-memory writes visible to the async proxy, then the group's barrier, then the copy.
+template <int NT>
+__device__ __forceinline__ void store_staged(char *g, const char *sb, uint32_t beg, uint32_t len, uint32_t phase)
 {
-    uint32_t saddr = (uint32_t)__cvta_generic_to_shared(ssrc);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" :: "l"(gdst), "r"(saddr), "r"(bytes) : "memory");
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    if (NT == 32) __syncwarp(); else __syncthreads();
+    const uint32_t lane = threadIdx.x % NT;
+    const uint32_t head = min(len, (16u - ((phase + beg) & 15u)) & 15u);
+    const uint32_t body = (len - head) & ~15u;
+    const uint32_t tail = len - head - body;
+    g += beg; sb += beg;
+    if (lane < head) g[lane] = sb[lane];
+    if (lane < tail) g[head + body + lane] = sb[head + body + lane];
+    if (body && lane == 0) {
+        asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" :: "l"(g + head), "r"((uint32_t)__cvta_generic_to_shared(sb + head)), "r"(body) : "memory");
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+    }
 }
 
 // ---- text kernels: no inter-CTA dependency at all ---------------------------
@@ -319,7 +212,7 @@ __device__ __forceinline__ void text_size_tile(const Fmt &fmt, int32_t ncols, ui
 
 template <class Fmt>
 __device__ __forceinline__ void text_write_tile(const Fmt &fmt, int32_t ncols, const uint32_t *len_in, const typename Fmt::State *st_in,
-                                                const uint64_t *tile_base, char *out, uint32_t smem_cap, int use_tma)
+                                                const uint64_t *tile_base, char *out, uint32_t smem_cap)
 {
     extern __shared__ __align__(16) char s_text[];
     __shared__ uint32_t s_ws[TILE / 32];
@@ -328,29 +221,14 @@ __device__ __forceinline__ void text_write_tile(const Fmt &fmt, int32_t ncols, c
     uint32_t len = 0;
     if (c < ncols) { len = len_in[c]; if (len) stt = st_in[c]; }
     uint32_t total;
-    const uint32_t off = block_excl_scan<TILE>(len, s_ws, total);
+    const uint32_t off = block_excl_scan<TILE, ScanSum>(len, s_ws, total);
     if (total == 0) return;
     const uint64_t base = tile_base[blockIdx.x];
     const uint32_t phase = (uint32_t)(base & 15);
     if (total + phase <= smem_cap) {
         char *sb = s_text + phase;
         if (len) fmt.write(c, stt, sb + off);
-        __syncthreads();
-        char *g = out + base;
-        const uint32_t head = min(total, (16u - phase) & 15u);
-        const uint32_t body = (total - head) & ~15u;
-        const uint32_t tail = total - head - body;
-        if (threadIdx.x < head) g[threadIdx.x] = sb[threadIdx.x];
-        if (threadIdx.x < tail) g[head + body + threadIdx.x] = sb[head + body + threadIdx.x];
-        if (body) {
-            if (use_tma) {
-                if (threadIdx.x == 0) bulk_store_s2g(g + head, sb + head, body);
-            } else {
-                const uint4 *src = reinterpret_cast<const uint4 *>(sb + head);
-                uint4 *dst = reinterpret_cast<uint4 *>(g + head);
-                for (uint32_t i = threadIdx.x; i < body / 16; i += TILE) dst[i] = src[i];
-            }
-        }
+        store_staged<TILE>(out + base, sb, 0, total, phase);
     } else if (len) {
         fmt.write(c, stt, out + base + off);
     }
@@ -368,9 +246,9 @@ __global__ void __launch_bounds__(TILE) k_mpileup_size(MpFmt fmt, uint32_t *len,
     text_size_tile(fmt, fmt.v.ncols, len, st, tile_total);
 }
 __global__ void __launch_bounds__(TILE) k_mpileup_write(MpFmt fmt, const uint32_t *len, const MpFileSz *st, const uint64_t *tile_base,
-                                                        char *out, uint32_t smem_cap, int use_tma)
+                                                        char *out, uint32_t smem_cap)
 {
-    text_write_tile(fmt, fmt.v.ncols, len, st, tile_base, out, smem_cap, use_tma);
+    text_write_tile(fmt, fmt.v.ncols, len, st, tile_base, out, smem_cap);
 }
 #include "mpileup_ss.cuh"
 #include "mpileup_ent.cuh"
@@ -387,9 +265,9 @@ __global__ void __launch_bounds__(TILE) k_depth_size(DpFmt fmt, uint32_t *len, D
     text_size_tile(fmt, fmt.v.ncols, len, st, tile_total);
 }
 __global__ void __launch_bounds__(TILE) k_depth_write(DpFmt fmt, const uint32_t *len, const DpFmt::State *st, const uint64_t *tile_base,
-                                                      char *out, uint32_t smem_cap, int use_tma)
+                                                      char *out, uint32_t smem_cap)
 {
-    text_write_tile(fmt, fmt.v.ncols, len, st, tile_base, out, smem_cap, use_tma);
+    text_write_tile(fmt, fmt.v.ncols, len, st, tile_base, out, smem_cap);
 }
 
 // coverage column sums (coverage.c:622-660)
@@ -469,39 +347,6 @@ __global__ void k_entries_fill(View v, int f, int32_t c0, const uint64_t *col_of
         *o++ = p;
     }
 }
-__global__ void k_scan_u32_to_u64(const uint32_t *in, uint64_t *out, int32_t n, uint64_t *st, uint32_t *ticket)
-{
-    constexpr int T = 256;
-    __shared__ uint32_t s_ws[T / 32];
-    __shared__ int s_tile; __shared__ uint64_t s_base;
-    if (threadIdx.x == 0) s_tile = (int)atomicAdd(ticket, 1u);
-    __syncthreads();
-    const int t = s_tile;
-    const int32_t i = t * T + (int32_t)threadIdx.x;
-    uint32_t v = i < n ? in[i] : 0, total;
-    uint32_t off = block_excl_scan<T>(v, s_ws, total);
-    if (threadIdx.x < 32) { const uint64_t b = lookback_sum(st, t, total); if (threadIdx.x == 0) s_base = b; }
-    __syncthreads();
-    if (i < n) out[i] = s_base + off;
-    if (i == n - 1) out[n] = s_base + off + v;
-}
-
-__global__ void k_scan_u32_excl_i32(const uint32_t *in, int32_t *out, int32_t n, uint64_t *st, uint32_t *ticket)
-{
-    constexpr int T = 256;
-    __shared__ uint32_t s_ws[T / 32];
-    __shared__ int s_tile; __shared__ uint64_t s_base;
-    if (threadIdx.x == 0) s_tile = (int)atomicAdd(ticket, 1u);
-    __syncthreads();
-    const int t = s_tile;
-    const int32_t i = t * T + (int32_t)threadIdx.x;
-    uint32_t v = i < n ? in[i] : 0, total;
-    uint32_t off = block_excl_scan<T>(v, s_ws, total);
-    if (threadIdx.x < 32) { const uint64_t b = lookback_sum(st, t, total); if (threadIdx.x == 0) s_base = b; }
-    __syncthreads();
-    if (i < n) out[i] = (int32_t)(s_base + off);
-    if (i == n - 1) out[n] = (int32_t)(s_base + off + v);
-}
 
 // ============================== host side ====================================
 template <class T> static int ensure(b200_engine *e, T *&p, size_t &cap, size_t need)
@@ -517,6 +362,28 @@ template <class T> static int ensure(b200_engine *e, T *&p, size_t &cap, size_t 
 #define ENSURE(field, need) do { if (ensure(e, e->field, e->cap_##field, (need))) return -1; } while (0)
 
 static inline int nblk(int64_t n, int t) { return (int)((n + t - 1) / t); }
+
+// Fresh look-back state for nb blocks of a single-pass scan (scan.cuh): the block ticket, then `arrays` arrays of nb status
+// words, zeroed by one memset
+static int lookback_state(b200_engine *e, int nb, int arrays, uint32_t **ticket, uint64_t **st)
+{
+    const size_t words = 1 + (size_t)arrays * nb;
+    ENSURE(status, words);
+    CK(cudaMemsetAsync(e->status, 0, words * 8, e->stream));
+    *ticket = (uint32_t *)e->status; *st = e->status + 1;
+    return 0;
+}
+// out[] = k_scan<Op, IPT, INCL> of in[0, n), n > 0
+template <class Op, int IPT, bool INCL, class In, class Out>
+static int launch_scan(b200_engine *e, const In *in, Out *out, int64_t n)
+{
+    if (n > INT32_MAX - SCAN_T * IPT) { snprintf(e->err, sizeof e->err, "scan of %lld items exceeds the 32-bit index range", (long long)n); return -1; }
+    const int nb = nblk(n, SCAN_T * IPT);
+    uint32_t *ticket; uint64_t *st;
+    if (lookback_state(e, nb, 1, &ticket, &st)) return -1;
+    k_scan<Op, IPT, INCL><<<nb, SCAN_T, 0, e->stream>>>(in, out, (int32_t)n, st, ticket); e->launches++;
+    return 0;
+}
 
 #include "overlap.cuh"
 #include "baq.cuh"
@@ -552,7 +419,6 @@ extern "C" int b200_engine_create(int device, b200_engine_t **out)
     cudaDeviceGetAttribute(&e->n_sm, cudaDevAttrMultiProcessorCount, device);
     e->smem_text = 24 * 1024;
     const char *s = getenv("B200_PLP_SMEM_TEXT"); if (s) e->smem_text = (uint32_t)atoi(s);
-    s = getenv("B200_PLP_TMA"); e->use_tma = s ? atoi(s) : 1;
     s = getenv("B200_PLP_GENERAL"); e->general = s ? atoi(s) : 0;   // 1: general mpileup path (thread-per-column size + write) for every configuration
     s = getenv("B200_BAQ_REG"); e->baq_reg = s ? atoi(s) : 1;
     if (e->smem_text + 16 > 48 * 1024) {   // the attribute is per function and process-wide: only ever raise it (another handle may use more)
@@ -615,20 +481,17 @@ static int max_buffered_reads(b200_engine *e, int *out)
 {
     const int32_t ncols = e->ncols_max + 1;
     ENSURE(ss_diff, (size_t)ncols + 3); ENSURE(ss_nplp, (size_t)ncols + 3);
-    const int nbs = nblk((int64_t)ncols + 2, 1024);
-    ENSURE(status2, (size_t)nbs + 1);
     int best = 0;
     for (int f = 0; f < e->n_files; ++f) {
         const int64_t i0 = e->h_file_start[f], i1 = e->h_file_start[f + 1];
         if (i1 <= i0) continue;
         CK(cudaMemsetAsync(e->ss_diff, 0, ((size_t)ncols + 2) * 4, e->stream));
-        CK(cudaMemsetAsync(e->status2, 0, ((size_t)nbs + 1) * 8, e->stream));
-        CK(cudaMemsetAsync(e->d_misc + 2, 0, 16, e->stream));
+        CK(cudaMemsetAsync(e->d_misc + MISC_MAX_BUFFERED, 0, 8, e->stream));
         k_cov_diff<<<nblk(i1 - i0, 256), 256, 0, e->stream>>>(e->state, e->desc, e->rlen, i0, i1, ncols, e->ss_diff); e->launches++;
-        k_ss_scan<<<nbs, 256, 0, e->stream>>>(e->ss_diff, e->ss_nplp, ncols + 2, e->status2, (uint32_t *)(e->d_misc + 2)); e->launches++;
-        k_max_i32<<<e->n_sm * 4, 256, 0, e->stream>>>(e->ss_nplp, ncols + 2, (int *)(e->d_misc + 3)); e->launches++;
+        if (launch_scan<ScanSum, 4, true>(e, e->ss_diff, e->ss_nplp, (int64_t)ncols + 2)) return -1;
+        k_max_i32<<<e->n_sm * 4, 256, 0, e->stream>>>(e->ss_nplp, ncols + 2, (int *)(e->d_misc + MISC_MAX_BUFFERED)); e->launches++;
         int m = 0;
-        CK(cudaMemcpyAsync(&m, e->d_misc + 3, 4, cudaMemcpyDeviceToHost, e->stream));
+        CK(cudaMemcpyAsync(&m, e->d_misc + MISC_MAX_BUFFERED, 4, cudaMemcpyDeviceToHost, e->stream));
         CK(cudaStreamSynchronize(e->stream));
         if (m > best) best = m;
     }
@@ -859,33 +722,22 @@ int build_ranges(b200_engine *e, int *max_range)
     // prefix max of read ends, file by file
     for (int f = 0; f < e->n_files; ++f) {
         const int64_t fs = e->h_file_start[f], fn = e->h_file_start[f + 1] - fs;
-        if (fn <= 0) continue;
-        const int nb = nblk(fn, 256 * 8);
-        ENSURE(status, (size_t)nb + 1);
-        CK(cudaMemsetAsync(e->status, 0, ((size_t)nb + 1) * 8, e->stream));
-        CK(cudaMemsetAsync(e->d_misc, 0, 8, e->stream));
-        k_scan_max<<<nb, 256, 0, e->stream>>>(e->endv + fs, e->pmax + fs, fn, e->status, (uint32_t *)e->d_misc); e->launches++;
+        if (fn > 0 && launch_scan<ScanMax, 8, true>(e, e->endv + fs, e->pmax + fs, fn)) return -1;
     }
-    CK(cudaMemsetAsync(e->d_misc + 1, 0, 8, e->stream));
+    CK(cudaMemsetAsync(e->d_misc + MISC_RANGE_MAX, 0, 8, e->stream));
     const int64_t tot = (int64_t)e->n_groups * e->n_files;
-    k_ranges<<<nblk(tot, 256), 256, 0, e->stream>>>(e->desc, e->pmax, e->file_start, e->n_files, e->n_groups, e->glo, e->ghi, (int *)(e->d_misc + 1));
+    k_ranges<<<nblk(tot, 256), 256, 0, e->stream>>>(e->desc, e->pmax, e->file_start, e->n_files, e->n_groups, e->glo, e->ghi, (int *)(e->d_misc + MISC_RANGE_MAX));
     e->launches++;
     // far-reaching reads per group
     ENSURE(ovf_cnt, (size_t)tot + 1); ENSURE(ovf_off, (size_t)tot + 2);
     CK(cudaMemsetAsync(e->ovf_cnt, 0, ((size_t)tot + 1) * 4, e->stream));
     k_ovf_count<<<nblk(n, 256), 256, 0, e->stream>>>(e->desc, e->file_start, e->n_files, n, e->n_groups, e->ovf_cnt); e->launches++;
-    k_ovf_max<<<nblk(tot, 256), 256, 0, e->stream>>>(e->ovf_cnt, tot, (int *)(e->d_misc + 1) + 1); e->launches++;
-    {
-        const int nb = nblk(tot, 256);
-        ENSURE(status, (size_t)nb + 1);
-        CK(cudaMemsetAsync(e->status, 0, ((size_t)nb + 1) * 8, e->stream));
-        CK(cudaMemsetAsync(e->d_misc, 0, 8, e->stream));
-        k_scan_u32_excl_i32<<<nb, 256, 0, e->stream>>>(e->ovf_cnt, e->ovf_off, (int32_t)tot, e->status, (uint32_t *)e->d_misc); e->launches++;
-    }
+    k_ovf_max<<<nblk(tot, 256), 256, 0, e->stream>>>(e->ovf_cnt, tot, (int *)(e->d_misc + MISC_RANGE_MAX) + 1); e->launches++;
+    if (launch_scan<ScanSum, 1, false>(e, e->ovf_cnt, e->ovf_off, tot)) return -1;
     int32_t n_ovf = 0;
     CK(cudaMemcpyAsync(&n_ovf, e->ovf_off + tot, 4, cudaMemcpyDeviceToHost, e->stream));
     int mx[2] = {0, 0};                        // widest slice, longest far-reaching list
-    CK(cudaMemcpyAsync(mx, e->d_misc + 1, sizeof mx, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(mx, e->d_misc + MISC_RANGE_MAX, sizeof mx, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     *max_range = column_read_bound(mx[0], mx[1]);
     ENSURE(ovf_idx, (size_t)n_ovf + 1);
@@ -920,49 +772,58 @@ static int upload_bed(b200_engine *e, const int64_t *bb, const int64_t *be, int 
     return 0;
 }
 
-template <class Fmt, class KS, class KW>
-static int run_text(b200_engine *e, KS k_size, KW k_write, const Fmt &fmt, uint64_t bound, char *out, size_t out_cap, size_t *out_len)
+// Start of a text call: nothing written yet and the text buffer sized for `bound`.  Returns the number of 128-column tiles
+// of the window (0: nothing to do), or -1.
+static int text_begin(b200_engine *e, int32_t ncols, uint64_t bound, size_t *out_len)
 {
-    const int32_t ncols = fmt.v.ncols;
+    *out_len = 0; e->last_kernel_ms = 0;
     const int nt = (ncols + TILE - 1) / TILE;
-    *out_len = 0;
-    e->last_kernel_ms = 0;
-    if (nt == 0) return 0;
-    ENSURE(out, (size_t)bound + 64);
+    if (nt) ENSURE(out, (size_t)bound + 64);
+    return nt;
+}
+
+// End of a text call whose three kernels were enqueued between the events ev0, evA, evB and ev1: reads back the text length
+// from *d_len, times the call and its three parts, checks the length against the bound and copies the text out.
+static int text_end(b200_engine *e, const uint64_t *d_len, uint64_t bound, char *out, size_t out_cap, size_t *out_len)
+{
     unsigned long long total = 0;
-    typedef typename Fmt::State State;
-    ENSURE(col_n, (size_t)ncols + 1);                                   // per-column line length
-    const size_t st_words = ((size_t)ncols * sizeof(State) + 7) / 8 + 1;
-    ENSURE(col_state, st_words);                                        // per-column formatter state
-    ENSURE(tile_total, (size_t)nt + 1); ENSURE(col_off, (size_t)nt + 2);
-    const int nb = nblk(nt, 256);
-    ENSURE(status, (size_t)nb + 1);
-    CK(cudaMemsetAsync(e->status, 0, ((size_t)nb + 1) * 8, e->stream));
-    CK(cudaMemsetAsync(e->d_misc, 0, 8, e->stream));
-    CK(cudaEventRecord(e->ev0, e->stream));
-    k_size<<<nt, TILE, 0, e->stream>>>(fmt, e->col_n, (State *)e->col_state, e->tile_total); e->launches++;
-    CK(cudaEventRecord(e->evA, e->stream));
-    k_scan_u32_to_u64<<<nb, 256, 0, e->stream>>>(e->tile_total, e->col_off, nt, e->status, (uint32_t *)e->d_misc); e->launches++;
-    CK(cudaEventRecord(e->evB, e->stream));
-    k_write<<<nt, TILE, e->smem_text + 16, e->stream>>>(fmt, e->col_n, (const State *)e->col_state, e->col_off, e->out, e->smem_text, e->use_tma);
-    e->launches++;
-    CK(cudaEventRecord(e->ev1, e->stream));
-    CK(cudaMemcpyAsync(&total, e->col_off + nt, 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(&total, d_len, 8, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     CK(cudaGetLastError());
+    const cudaEvent_t ev[4] = {e->ev0, e->evA, e->evB, e->ev1};
     float ms = 0; cudaEventElapsedTime(&ms, e->ev0, e->ev1); e->last_kernel_ms = ms;
-    cudaEventElapsedTime(&ms, e->ev0, e->evA); e->last_parts_ms[0] = ms;      // size pass
-    cudaEventElapsedTime(&ms, e->evA, e->evB); e->last_parts_ms[1] = ms;      // tile-offset scan
-    cudaEventElapsedTime(&ms, e->evB, e->ev1); e->last_parts_ms[2] = ms;      // write pass
+    for (int k = 0; k < 3; ++k) { cudaEventElapsedTime(&ms, ev[k], ev[k + 1]); e->last_parts_ms[k] = ms; }
     if (total > bound) { snprintf(e->err, sizeof e->err, "internal: output %llu exceeds bound %llu", total, (unsigned long long)bound); return -1; }
-    *out_len = (size_t)total;
-    e->last_out_len = (size_t)total;
+    *out_len = (size_t)total; e->last_out_len = (size_t)total;
     if (out) {
         if (total > out_cap) { snprintf(e->err, sizeof e->err, "output buffer too small: need %llu bytes", total); return -2; }
         CK(cudaMemcpyAsync(out, e->out, (size_t)total, cudaMemcpyDeviceToHost, e->stream));
         CK(cudaStreamSynchronize(e->stream));
     }
     return 0;
+}
+
+// thread-per-column text: size pass, tile-offset scan and write pass are the three timed parts
+template <class Fmt, class KS, class KW>
+static int run_text(b200_engine *e, KS k_size, KW k_write, const Fmt &fmt, uint64_t bound, char *out, size_t out_cap, size_t *out_len)
+{
+    const int32_t ncols = fmt.v.ncols;
+    const int nt = text_begin(e, ncols, bound, out_len);
+    if (nt <= 0) return nt;
+    typedef typename Fmt::State State;
+    ENSURE(col_n, (size_t)ncols + 1);                                   // per-column line length
+    const size_t st_words = ((size_t)ncols * sizeof(State) + 7) / 8 + 1;
+    ENSURE(col_state, st_words);                                        // per-column formatter state
+    ENSURE(tile_total, (size_t)nt + 1); ENSURE(col_off, (size_t)nt + 2);
+    CK(cudaEventRecord(e->ev0, e->stream));
+    k_size<<<nt, TILE, 0, e->stream>>>(fmt, e->col_n, (State *)e->col_state, e->tile_total); e->launches++;
+    CK(cudaEventRecord(e->evA, e->stream));
+    if (launch_scan<ScanSum, 1, false>(e, e->tile_total, e->col_off, nt)) return -1;
+    CK(cudaEventRecord(e->evB, e->stream));
+    k_write<<<nt, TILE, e->smem_text + 16, e->stream>>>(fmt, e->col_n, (const State *)e->col_state, e->col_off, e->out, e->smem_text);
+    e->launches++;
+    CK(cudaEventRecord(e->ev1, e->stream));
+    return text_end(e, e->col_off + nt, bound, out, out_cap, out_len);
 }
 
 extern "C" uint64_t b200_mpileup_text_bound(const b200_engine_t *e, const b200_mpileup_conf_t *c)
@@ -990,35 +851,33 @@ extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c,
     if (e->general || e->n_files != 1 || c->out_qpos || c->out_qpos5 || c->n_x > 0)
         return run_text(e, k_mpileup_size, k_mpileup_write, fmt, bound, out, out_cap, out_len);
     // ---- default (one input file, no -O columns): entry strings + gather (mpileup_ent.cuh)
+    // the three timed parts: k_mp_entries (entry strings + line-length sums), k_mp_place (n_plp, line lengths, tile offsets),
+    // k_mp_gather
     const int32_t ncols = fmt.v.ncols;
-    const int nt = (ncols + TILE - 1) / TILE;            // 128-column tiles
-    *out_len = 0; e->last_kernel_ms = 0;
-    if (nt == 0) return 0;
-    ENSURE(out, (size_t)bound + 64);
+    const int nt = text_begin(e, ncols, bound, out_len);
+    if (nt <= 0) return nt;
     ENSURE(col_off, (size_t)nt + 2);
     ENSURE(ent, e->qual_bytes + 64 + ENT_PAD); ENSURE(ent2, (size_t)e->sum_rlen_gen + 64 + ENT_PAD);   // front pad + slack for the gather's 80-byte fetches
     ENSURE(ss_diff, (size_t)ncols + 3); ENSURE(ss_nplp, (size_t)ncols + 2); ENSURE(ss_fail, (size_t)ncols + 3); ENSURE(ss_extra, (size_t)ncols + 3);   // k_mp_place reads up to ncols + 2
     CK(cudaMemsetAsync(e->ss_diff, 0, ((size_t)ncols + 2) * 4, e->stream));
     CK(cudaMemsetAsync(e->ss_fail, 0, ((size_t)ncols + 1) * 4, e->stream));
     CK(cudaMemsetAsync(e->ss_extra, 0, ((size_t)ncols + 1) * 4, e->stream));
-    const int nbp = nblk(ncols, PLACE_COLS);                // k_mp_place blocks; look-back status: coverage (status2), bytes (status)
-    ENSURE(status, (size_t)nbp + 1); ENSURE(status2, (size_t)nbp + 1);
-    CK(cudaMemsetAsync(e->status, 0, ((size_t)nbp + 1) * 8, e->stream));
-    CK(cudaMemsetAsync(e->status2, 0, ((size_t)nbp + 1) * 8, e->stream));
-    CK(cudaMemsetAsync(e->d_misc + 2, 0, 16, e->stream));      // k_mp_place ticket, cursor of the second entry array
+    const int nbp = nblk(ncols, PLACE_COLS);                // k_mp_place blocks; look-back status: coverage, then bytes
+    uint32_t *ticket; uint64_t *st;
+    if (lookback_state(e, nbp, 2, &ticket, &st)) return -1;
+    CK(cudaMemsetAsync(e->d_misc + MISC_ENT2_CURSOR, 0, 8, e->stream));
     CK(cudaEventRecord(e->ev0, e->stream));
     {
         // one warp per 32 reads, 8 warps per block; up to 64 blocks per SM, so that an 8 Mb window at 30x (1.6 M reads) runs in
         // one pass instead of three grid-stride rounds (5 % faster than 16 per SM: no partly filled last round)
         const int64_t want_blocks = (e->n + 255) / 256;
         const int rb = (int)std::max<int64_t>(1, std::min<int64_t>(want_blocks, (int64_t)e->n_sm * 64));
-        if (e->has_ref) k_mp_entries<true><<<rb, 256, 0, e->stream>>>(fmt.v, fmt.cf, e->n, e->ref_codes, e->ss_diff, e->ss_fail, e->ss_extra, e->ent + ENT_PAD, e->ent2 + ENT_PAD, e->d_misc + 3, e->desc);
-        else k_mp_entries<false><<<rb, 256, 0, e->stream>>>(fmt.v, fmt.cf, e->n, nullptr, e->ss_diff, e->ss_fail, e->ss_extra, e->ent + ENT_PAD, e->ent2 + ENT_PAD, e->d_misc + 3, e->desc);
+        if (e->has_ref) k_mp_entries<true><<<rb, 256, 0, e->stream>>>(fmt.v, fmt.cf, e->n, e->ref_codes, e->ss_diff, e->ss_fail, e->ss_extra, e->ent + ENT_PAD, e->ent2 + ENT_PAD, e->d_misc + MISC_ENT2_CURSOR, e->desc);
+        else k_mp_entries<false><<<rb, 256, 0, e->stream>>>(fmt.v, fmt.cf, e->n, nullptr, e->ss_diff, e->ss_fail, e->ss_extra, e->ent + ENT_PAD, e->ent2 + ENT_PAD, e->d_misc + MISC_ENT2_CURSOR, e->desc);
         e->launches++;
     }
     CK(cudaEventRecord(e->evA, e->stream));
-    k_mp_place<<<nbp, 256, 0, e->stream>>>(fmt.v, fmt.cf, e->ss_diff, e->ss_fail, e->ss_extra, e->ss_nplp, e->col_off, nt, e->status2, e->status,
-                                            (uint32_t *)(e->d_misc + 2)); e->launches++;
+    k_mp_place<<<nbp, 256, 0, e->stream>>>(fmt.v, fmt.cf, e->ss_diff, e->ss_fail, e->ss_extra, e->ss_nplp, e->col_off, nt, st, st + nbp, ticket); e->launches++;
     CK(cudaEventRecord(e->evB, e->stream));
     {
         MpEntFmt gf; gf.v = fmt.v; gf.cf = fmt.cf; gf.E = e->ent + ENT_PAD; gf.E2 = e->ent2 + ENT_PAD;
@@ -1035,27 +894,12 @@ extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c,
             const uint64_t want = std::max<uint64_t>(12 * 1024, (avg_tile * 9 / 8 + 1023) & ~1023ull);
             if (want < cap) cap = (uint32_t)want;
         }
-        if (c->out_mapq) k_mp_gather<7, true><<<nt, TILE, cap + 16, e->stream>>>(gf, dg, e->ss_nplp, e->ss_fail, e->ss_extra, e->col_off, e->out, cap, e->use_tma);
-        else k_mp_gather<7, false><<<nt, TILE, cap + 16, e->stream>>>(gf, dg, e->ss_nplp, e->ss_fail, e->ss_extra, e->col_off, e->out, cap, e->use_tma);
+        if (c->out_mapq) k_mp_gather<7, true><<<nt, TILE, cap + 16, e->stream>>>(gf, dg, e->ss_nplp, e->ss_fail, e->ss_extra, e->col_off, e->out, cap);
+        else k_mp_gather<7, false><<<nt, TILE, cap + 16, e->stream>>>(gf, dg, e->ss_nplp, e->ss_fail, e->ss_extra, e->col_off, e->out, cap);
         e->launches++;
     }
     CK(cudaEventRecord(e->ev1, e->stream));
-    unsigned long long total = 0;
-    CK(cudaMemcpyAsync(&total, e->col_off + nt, 8, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
-    CK(cudaGetLastError());
-    float ms = 0; cudaEventElapsedTime(&ms, e->ev0, e->ev1); e->last_kernel_ms = ms;
-    cudaEventElapsedTime(&ms, e->ev0, e->evA); e->last_parts_ms[0] = ms;      // k_mp_entries: entry strings + line-length sums
-    cudaEventElapsedTime(&ms, e->evA, e->evB); e->last_parts_ms[1] = ms;      // k_mp_place: n_plp, line lengths, tile offsets
-    cudaEventElapsedTime(&ms, e->evB, e->ev1); e->last_parts_ms[2] = ms;      // k_mp_gather
-    if (total > bound) { snprintf(e->err, sizeof e->err, "internal: output %llu exceeds bound %llu", total, (unsigned long long)bound); return -1; }
-    *out_len = (size_t)total; e->last_out_len = (size_t)total;
-    if (out) {
-        if (total > out_cap) { snprintf(e->err, sizeof e->err, "output buffer too small: need %llu bytes", total); return -2; }
-        CK(cudaMemcpyAsync(out, e->out, (size_t)total, cudaMemcpyDeviceToHost, e->stream));
-        CK(cudaStreamSynchronize(e->stream));
-    }
-    return 0;
+    return text_end(e, e->col_off + nt, bound, out, out_cap, out_len);
 }
 
 extern "C" int b200_depth_text(b200_engine_t *e, const b200_depth_conf_t *c, char *out, size_t out_cap, size_t *out_len)
@@ -1079,12 +923,12 @@ extern "C" int b200_coverage(b200_engine_t *e, const b200_coverage_conf_t *c, b2
     CK(cudaSetDevice(e->device));
     View v; fill_view(e, v, nullptr, nullptr, 0, 0, 0);
     memset(sums, 0, sizeof *sums);
-    CK(cudaMemsetAsync(e->d_misc + 8, 0, 5 * 8, e->stream));
+    CK(cudaMemsetAsync(e->d_misc + MISC_COVERAGE, 0, 5 * 8, e->stream));
     CK(cudaEventRecord(e->ev0, e->stream));
-    if (v.ncols > 0) { k_coverage<<<nblk(v.ncols, 256), 256, 0, e->stream>>>(v, c->min_baseQ, c->min_depth, e->d_misc + 8); e->launches++; }
+    if (v.ncols > 0) { k_coverage<<<nblk(v.ncols, 256), 256, 0, e->stream>>>(v, c->min_baseQ, c->min_depth, e->d_misc + MISC_COVERAGE); e->launches++; }
     CK(cudaEventRecord(e->ev1, e->stream));
     unsigned long long h[5];
-    CK(cudaMemcpyAsync(h, e->d_misc + 8, sizeof h, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(h, e->d_misc + MISC_COVERAGE, sizeof h, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     CK(cudaGetLastError());
     float ms = 0; cudaEventElapsedTime(&ms, e->ev0, e->ev1); e->last_kernel_ms = ms;
@@ -1167,11 +1011,7 @@ extern "C" int b200_pileup_entries(b200_engine_t *e, int32_t file, int64_t beg, 
     const int64_t nc = re - rb;
     ENSURE(col_n, (size_t)nc + 1); ENSURE(col_off, (size_t)nc + 2);
     k_entries_count<<<nblk(nc, 256), 256, 0, e->stream>>>(v, file, (int32_t)rb, e->col_n); e->launches++;
-    const int nb = nblk(nc, 256);
-    ENSURE(status, (size_t)nb + 1);
-    CK(cudaMemsetAsync(e->status, 0, ((size_t)nb + 1) * 8, e->stream));
-    CK(cudaMemsetAsync(e->d_misc, 0, 8, e->stream));
-    k_scan_u32_to_u64<<<nb, 256, 0, e->stream>>>(e->col_n, e->col_off, (int32_t)nc, e->status, (uint32_t *)e->d_misc); e->launches++;
+    if (launch_scan<ScanSum, 1, false>(e, e->col_n, e->col_off, nc)) return -1;
     uint64_t tot = 0;
     CK(cudaMemcpyAsync(&tot, e->col_off + nc, 8, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));

@@ -242,11 +242,7 @@ extern "C" int b200_glf(b200_engine_t *e, int32_t min_baseQ, int64_t *n_cols, in
     CK(cudaMemsetAsync(e->gl_flag, 0, ((size_t)v.ncols + 2) * 4, e->stream));
     CK(cudaEventRecord(e->ev0, e->stream));
     k_gl_count<<<nblk(tot, 256), 256, 0, e->stream>>>(v, min_baseQ, e->col_n, (int32_t *)e->gl_flag); e->launches++;
-    const int nb = nblk(tot, 256);
-    ENSURE(status, (size_t)nb + 1);
-    CK(cudaMemsetAsync(e->status, 0, ((size_t)nb + 1) * 8, e->stream));
-    CK(cudaMemsetAsync(e->d_misc, 0, 8, e->stream));
-    k_scan_u32_to_u64<<<nb, 256, 0, e->stream>>>(e->col_n, e->col_off, (int32_t)tot, e->status, (uint32_t *)e->d_misc); e->launches++;
+    if (launch_scan<ScanSum, 1, false>(e, e->col_n, e->col_off, tot)) return -1;
     uint32_t *ovf = (uint32_t *)(e->gl_flag + v.ncols);
     k_gl<<<nblk(tot * 32, 128), 128, 0, e->stream>>>(v, min_baseQ, e->col_off, e->gl_rng_draws, e->d_fk, e->d_beta, e->d_lhet,
                                                     e->gl_n, e->gl_out, ovf); e->launches++;

@@ -367,7 +367,7 @@ __device__ __forceinline__ void gather_group(const MpEntFmt &fmt, const MpEntFmt
 
 template <int MIN_CTAS, bool OUT_MAPQ>
 __global__ void __launch_bounds__(TILE, MIN_CTAS) k_mp_gather(MpEntFmt fmt, const MpEntFmt *gfmt, const int32_t *nplp, const uint32_t *fail, const uint32_t *extra,
-                                                              const uint64_t *tile_base, char *out, uint32_t smem_cap, int use_tma)
+                                                              const uint64_t *tile_base, char *out, uint32_t smem_cap)
 {
     extern __shared__ __align__(16) char s_text[];
     __shared__ uint32_t s_ws[TILE / 32];
@@ -386,13 +386,13 @@ __global__ void __launch_bounds__(TILE, MIN_CTAS) k_mp_gather(MpEntFmt fmt, cons
     MpFileSz stt;
     const uint32_t len = c < ncols ? mp_sums_line_size(fmt.v, fmt.cf, c, np, nf, nx, &stt) : 0u;
     uint32_t total;
-    const uint32_t off = block_excl_scan<TILE>(len, s_ws, total);
+    const uint32_t off = block_excl_scan<TILE, ScanSum>(len, s_ws, total);
     if (total == 0) return;
     const uint32_t phase = (uint32_t)(base & 15);
     if (total + phase <= smem_cap) {
         char *sb = s_text + phase;
         // every line's fixed parts (header, count, separators, place holders, newline) by the column's own thread ...
-        const int wi = threadIdx.x >> 5, lane = threadIdx.x & 31;
+        const int wi = threadIdx.x >> 5;
         uint32_t so = 0, qo = 0, mo = 0;
         bool on = false;
         if (len) {
@@ -402,31 +402,10 @@ __global__ void __launch_bounds__(TILE, MIN_CTAS) k_mp_gather(MpEntFmt fmt, cons
         // ... then the entries of the warp's 32 columns
         if (__any_sync(0xffffffffu, on)) gather_group<OUT_MAPQ>(fmt, gfmt, rr, c0, on, so, qo, mo, sb, s_rows[wi], s_hdr[wi]);
         // Each warp stores its own 32 lines (contiguous in the tile) as soon as it has them: no block-wide barrier at the end,
-        // so a warp with a deep column does not hold the other three.  Ragged head (to the next 16 B boundary of the
-        // destination) and tail by the lanes, the aligned body through one TMA bulk store (shared memory is laid out with the
-        // destination's 16-byte phase).
+        // so a warp with a deep column does not hold the other three.
         const uint32_t wbeg = __shfl_sync(0xffffffffu, off, 0);
         const uint32_t wend = __shfl_sync(0xffffffffu, off + len, 31);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // this lane's text bytes -> visible to the bulk-copy engine
-        __syncwarp();
-        if (wend > wbeg) {
-            char *g = out + base;
-            const uint32_t wlen = wend - wbeg;
-            const uint32_t head = min(wlen, (16u - ((phase + wbeg) & 15u)) & 15u);
-            const uint32_t body = (wlen - head) & ~15u;
-            const uint32_t tail = wlen - head - body;
-            if ((uint32_t)lane < head) g[wbeg + lane] = sb[wbeg + lane];
-            if ((uint32_t)lane < tail) g[wbeg + head + body + lane] = sb[wbeg + head + body + lane];
-            if (body) {
-                if (use_tma) {
-                    if (lane == 0) bulk_store_s2g(g + wbeg + head, sb + wbeg + head, body);
-                } else {
-                    const uint4 *src = reinterpret_cast<const uint4 *>(sb + wbeg + head);
-                    uint4 *dst = reinterpret_cast<uint4 *>(g + wbeg + head);
-                    for (uint32_t i = lane; i < body / 16; i += 32) dst[i] = src[i];
-                }
-            }
-        }
+        store_staged<32>(out + base, sb, wbeg, wend - wbeg, phase);
     } else if (len) {
         mp_line_write_ent(gfmt->v, gfmt->cf, c, stt, out + base + off, gfmt->E, gfmt->E2);   // very deep tile: format straight into HBM
     }

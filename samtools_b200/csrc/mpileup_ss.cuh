@@ -7,32 +7,11 @@
 //   k_mp_entries (mpileup_ent.cuh) one warp per 32 reads, lanes over their bases: a coverage difference array gets
 //                +1/-1 per read, only FAILING bases and special entries touch per-column counters (sparse atomics)
 //   k_mp_place   one pass over the sums: prefix sum of the difference array -> n_plp per column, the line length of every
-//                column (plp_core.h mp_sums_line_size), and the byte offset of every 128-column tile of the gather
+//                column (plp_core.h mp_sums_line_size), and the byte offset of every 128-column tile of the gather; both
+//                prefixes cross blocks through the look-back of scan.cuh
 // The gather re-derives each column's length and state from the same three sums, so no per-column line state is stored.
 // Equivalent to mp_line_size (the general path); `test_c2_size_properties` checks that both paths agree.
 #pragma once
-
-// inclusive prefix sum of int32 (coverage), single pass with decoupled look-back
-__global__ void k_ss_scan(const int32_t *in, int32_t *out, int32_t n, uint64_t *st, uint32_t *ticket)
-{
-    constexpr int T = 256, IPT = 4;
-    __shared__ uint32_t s_ws[T / 32];
-    __shared__ int s_tile; __shared__ uint64_t s_base;
-    if (threadIdx.x == 0) s_tile = (int)atomicAdd(ticket, 1u);
-    __syncthreads();
-    const int t = s_tile;
-    const int32_t i0 = (t * T + (int32_t)threadIdx.x) * IPT;
-    int32_t x[IPT]; uint32_t sum = 0;
-#pragma unroll
-    for (int j = 0; j < IPT; ++j) { x[j] = i0 + j < n ? in[i0 + j] : 0; sum += (uint32_t)x[j]; x[j] = (int32_t)sum; }   // mod-2^32 arithmetic: partial sums may be negative
-    uint32_t total;
-    const uint32_t off = block_excl_scan<T>(sum, s_ws, total);
-    if (threadIdx.x < 32) { const uint64_t b = lookback_sum(st, t, (uint64_t)total); if (threadIdx.x == 0) s_base = b; }
-    __syncthreads();
-    const uint32_t base = (uint32_t)s_base + off;
-#pragma unroll
-    for (int j = 0; j < IPT; ++j) if (i0 + j < n) out[i0 + j] = (int32_t)(base + (uint32_t)x[j]);
-}
 
 // Sizes and places the gather's tiles.  A block owns PLACE_COLS consecutive columns (PLACE_COLS / TILE tiles).  It is bound by
 // the latency of its round trips (ticket, loads, two look-backs), not by bandwidth, so what sets its speed is how many
@@ -40,8 +19,8 @@ __global__ void k_ss_scan(const int32_t *in, int32_t *out, int32_t n, uint64_t *
 // 24 registers per thread), eight blocks of 2048 columns per SM.  Then PLACE_ROUNDS rounds of 256 consecutive columns, one
 // column per thread (conflict-free 4-byte shared-memory loads); the block's warp segments of 32 columns are in column order
 // at index round * 8 + warp, so one warp scans them for the block.  Blocks are ticketed: the predecessors a look-back waits
-// on have started.  Two look-backs: the coverage difference total (st_cov; mod-2^32 like k_ss_scan, since partial sums of
-// the difference array can be negative) gives n_plp, the byte total (st_len) the tile offsets.  Outputs: nplp[c] for
+// on have started.  Two look-backs: the coverage difference total (st_cov; mod-2^32 as ScanSum in scan.cuh, since partial
+// sums of the difference array can be negative) gives n_plp, the byte total (st_len) the tile offsets.  Outputs: nplp[c] for
 // c < ncols, col_off[t] for every tile t < nt, and col_off[nt], the text length, from the block that owns the last tile.
 // The three input arrays must be readable up to column ncols + 2 (they are: the entry pass writes diff[ncols]).
 constexpr int PLACE_ROUNDS = 8, PLACE_COLS = 256 * PLACE_ROUNDS;
@@ -90,7 +69,7 @@ __global__ void __launch_bounds__(256) k_mp_place(View v, MpConf cf, const int32
         uint32_t s = pair;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, s, o); if (lane >= o) s += y; }
-        const uint32_t base = (uint32_t)lookback_sum(st_cov, t, (uint64_t)__shfl_sync(0xffffffffu, s, 31));
+        const uint32_t base = (uint32_t)lookback<ScanSum>(st_cov, t, (uint64_t)__shfl_sync(0xffffffffu, s, 31));
         const uint32_t e = base + s - pair;
         s_cov[2 * lane] = e; s_cov[2 * lane + 1] = e + a;
     }
@@ -123,7 +102,7 @@ __global__ void __launch_bounds__(256) k_mp_place(View v, MpConf cf, const int32
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) { const uint64_t y = __shfl_up_sync(0xffffffffu, s, o); if (lane >= o) s += y; }
         const uint64_t total = __shfl_sync(0xffffffffu, s, 31);
-        const uint64_t base = lookback_sum(st_len, t, total);
+        const uint64_t base = lookback<ScanSum>(st_len, t, total);
         const int32_t tile0 = t * NTILE, tile = tile0 + lane;
         if (lane < NTILE && tile < nt) col_off[tile] = base + s - tl;
         if (lane == 0 && tile0 <= nt - 1 && nt - 1 < tile0 + NTILE) col_off[nt] = base + total;

@@ -69,10 +69,10 @@ int launch_overlap(b200_engine *e, const RawSoA &r)
 {
     if (link_chains(e, r)) return -1;
     if (ensure(e, e->ov_pairs, e->cap_ov_pairs, (size_t)r.n + 2)) return -1;      // at most n/2 pairs of two indices
-    CK(cudaMemsetAsync(e->d_misc + 40, 0, 8, e->stream));
-    k_overlap<<<nblk(r.n, 128), 128, 0, e->stream>>>(r, e->next, e->state, e->rlen, e->file_start, e->n_files, e->ov_pairs, (unsigned int *)(e->d_misc + 40)); e->launches++;
+    CK(cudaMemsetAsync(e->d_misc + MISC_OVERLAP, 0, 8, e->stream));
+    k_overlap<<<nblk(r.n, 128), 128, 0, e->stream>>>(r, e->next, e->state, e->rlen, e->file_start, e->n_files, e->ov_pairs, (unsigned int *)(e->d_misc + MISC_OVERLAP)); e->launches++;
     const int gt = (int)std::min<int64_t>(nblk((r.n / 2 + 1) * 32, 128), (int64_t)e->n_sm * 16);
-    k_overlap_tweak<<<gt, 128, 0, e->stream>>>(r, e->desc, e->rlen, e->ov_pairs, (const unsigned int *)(e->d_misc + 40)); e->launches++;
+    k_overlap_tweak<<<gt, 128, 0, e->stream>>>(r, e->desc, e->rlen, e->ov_pairs, (const unsigned int *)(e->d_misc + MISC_OVERLAP)); e->launches++;
     CK(cudaGetLastError());
     return 0;
 }

@@ -66,7 +66,7 @@ static RawSoA raw(b200_engine *e)
     return r;
 }
 
-// per-group read slices and far-reaching lists: the loops of k_scan_max, k_ranges and k_ovf_* (engine.cu) around the same
+// per-group read slices and far-reaching lists: the loops of the prefix-max scan, k_ranges and k_ovf_* (engine.cu) around the same
 // plp_stage.h rules; returns the bound on the reads of one file over one column
 static int build_ranges(b200_engine *e)
 {

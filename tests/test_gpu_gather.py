@@ -13,8 +13,8 @@ average tile:
   reach     deletions and N skips longer than 512 bases over a stacked group: far-reaching reads (listed ahead of the
             slice proper), plus one that starts inside the reach window.
 Compared as `mpileup -a` at -Q 0 and -Q 13, with -s, and with a FASTA (-B -f), with the engine created under the
-default environment, with the vectorised store instead of TMA (B200_PLP_TMA=0), with the direct-to-HBM path for every
-tile (B200_PLP_SMEM_TEXT=1024) and with a budget large enough for the 2000-read stack (B200_PLP_SMEM_TEXT=196608)."""
+default environment, with the direct-to-HBM path for every tile (B200_PLP_SMEM_TEXT=1024) and with a budget large enough
+for the 2000-read stack (B200_PLP_SMEM_TEXT=196608)."""
 import subprocess
 import numpy as np
 import pytest
@@ -25,7 +25,7 @@ pytestmark = pytest.mark.gpu
 M, I, D, N, S = 0, 1, 2, 3, 4
 STACKS = [1, 31, 32, 33, 63, 64, 65, 127, 128, 129, 2000]
 E2_AT = (0, 31, 32, 63, 64, 65)
-ENVS = {'default': {}, 'no_tma': {'B200_PLP_TMA': '0'}, 'direct': {'B200_PLP_SMEM_TEXT': '1024'},
+ENVS = {'default': {}, 'direct': {'B200_PLP_SMEM_TEXT': '1024'},
         'wide': {'B200_PLP_SMEM_TEXT': '196608'}}
 CONFS = [(['-Q', '0'], {'min_baseQ': 0}, False), (['-Q', '13'], {'min_baseQ': 13}, False),
          (['-s'], {'out_mapq': 1}, False), (['-B', '-f', 'ref.fa'], {}, True)]

@@ -132,8 +132,8 @@ def test_cli_long_noBAQ_options(long_dir, oracle_bin):
     assert not bad, bad[:3]
 
 
-@pytest.mark.parametrize('env', [{}, {'B200_PLP_SMEM_TEXT': '204000'}, {'B200_PLP_SMEM_TEXT': '204000', 'B200_PLP_GENERAL': '1'},
-                                 {'B200_PLP_SMEM_TEXT': '204000', 'B200_PLP_TMA': '0'}], ids=['default', 'smem204000', 'general', 'notma'])
+@pytest.mark.parametrize('env', [{}, {'B200_PLP_SMEM_TEXT': '204000'}, {'B200_PLP_SMEM_TEXT': '204000', 'B200_PLP_GENERAL': '1'}],
+                         ids=['default', 'smem204000', 'general'])
 def test_entry_longer_than_64k(env, long_dir, oracle_bin):
     """a 70 000-base deletion: its mpileup entry carries 70 000 deleted reference bases.  The tile's shared-memory text budget
     is 9/8 of the average tile's bound, at most B200_PLP_SMEM_TEXT: with a region of a few dozen columns around the deletion

@@ -197,7 +197,7 @@ def test_c2_size_properties():
     from samtools_b200 import engine, synth
     soa = noref(synth.make_batch(length=1_000_000, depth=30, seed=2))
     digests = {}
-    for tag, env in (('tma', {'B200_PLP_TMA': '1'}), ('vec', {'B200_PLP_TMA': '0'}), ('direct', {'B200_PLP_SMEM_TEXT': '1024'}),
+    for tag, env in (('default', {}), ('direct', {'B200_PLP_SMEM_TEXT': '1024'}),
                      ('general', {'B200_PLP_GENERAL': '1'}), ('general_direct', {'B200_PLP_GENERAL': '1', 'B200_PLP_SMEM_TEXT': '1024'})):
         os.environ.update(env)
         e = engine.Engine(0)
@@ -208,14 +208,14 @@ def test_c2_size_properties():
             os.environ.pop(k)
         assert t1 == t2, 'not idempotent'
         digests[tag] = hashlib.sha256(t1).hexdigest()
-        if tag == 'tma':
+        if tag == 'default':
             lines = t1.split(b'\n')
             assert len(lines) - 1 == 1_000_000                      # -a: one row per reference position
             assert lines[0].startswith(b'chr1\t1\tN\t') and lines[999_999].startswith(b'chr1\t1000000\tN\t')
             # depth column sums to the number of kept (read, column) pairs that pass -Q13; positions ascend
             pos = np.array([int(l.split(b'\t', 2)[1]) for l in lines[:-1:997]])
             assert (np.diff(pos) > 0).all()
-    assert len(set(digests.values())) == 1, digests   # entry-string path / general path, TMA / vector / direct-to-HBM stores all agree
+    assert len(set(digests.values())) == 1, digests   # entry-string path / general path, TMA / direct-to-HBM stores all agree
 
 
 # ---------------------------------------------------------------- BASELINE C2 size, CUDA bytes vs the oracle's bytes

@@ -1,7 +1,7 @@
 """A/B timing of engine variants in ONE process launch per variant (development aid; keeps GPU runs short).
 
   python tools/ab_probe.py [--mb 8] [--reps 5] [--profile] label[:ENV=V[,ENV=V...]] ...
-  e.g.  python tools/ab_probe.py default general:B200_PLP_GENERAL=1 vec:B200_PLP_TMA=0
+  e.g.  python tools/ab_probe.py default general:B200_PLP_GENERAL=1 direct:B200_PLP_SMEM_TEXT=1024
 
 Each variant runs in its own subprocess (the engine reads its environment at creation) on the bench workload
 (synthetic region, 30x, 150 bp, `mpileup -a`, no FASTA) and reports CUDA-event times of the read stage (device
