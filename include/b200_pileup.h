@@ -24,6 +24,7 @@
  *   b200_coverage_hist()  per-bin counters of -m / -D     coverage.c:609-660
  *   b200_bedcov()         per-interval column reducers    bedcov.c:303-331
  *   b200_glf()            bcf_call_glfgen + errmod_cal    bam2bcf.c:65-123 (+ htslib errmod.c)
+ *   b200_mpileup_counts() pileup_seq, as numbers           bam_plcmd.c:54-169 -> per-column strand-split base / indel counts
  *   b200_pileup_entries() bam_plp64_next/resolve_cigar2   (htslib sam.c) -> arrays of bam_pileup1_t fields
  *
  * Conventions: plain C, caller-owned host buffers, int return codes (0 ok,
@@ -220,6 +221,18 @@ int b200_bedcov(b200_engine_t *e, int32_t skip_del_refskip, int32_t min_depth, u
  * HBM (device-only timing, like out == NULL of the text calls); *n_cols is then the number of candidate columns */
 int b200_glf(b200_engine_t *e, int32_t min_baseQ, int64_t *n_cols, int64_t *col_pos, int32_t *n_bases,
              float *qsum, float *p25, size_t cap_cols);
+/* per-column base and indel counts of the mpileup column stage: what a parser of the `mpileup --reverse-del` text of the
+ * staged window counts, without the text.  Per file 19 uint32 planes of n_cols columns, planar: out[(f * 19 + k) * n + c]
+ * for column c = position - window start, c in [0, n) (the columns b200_mpileup_text() formats with all = 1; empty ones are
+ * zero).  Planes k = 0..8 count forward-strand entries, 9..17 reverse-strand ones, each as
+ *   0-3 A C G T (a '.' / ',' counts as the column's reference base)   4 any other base (also '.' / ',' without an A/C/G/T
+ *   reference)   5 deletion ('*' / '#')   6 reference skip ('>' / '<')   7 a "+n" insertion follows   8 a "-n" deletion follows
+ * counting only entries that pass -Q (min_baseQ, as in the text); plane 18 is n_plp, the reads over the column before -Q.
+ * out == NULL: compute only, the planes stay in HBM (device-only timing, like out == NULL of the text calls).  Otherwise out
+ * is host or device memory (a device buffer must be on the handle's device) of at least n_files * 19 * cap_cols words;
+ * cap_cols < n returns -2.  *n_cols always receives n.  Needs a batch staged in B200_MODE_MPILEUP. */
+#define B200_COUNT_PLANES 19
+int b200_mpileup_counts(b200_engine_t *e, int32_t min_baseQ, uint32_t *out, size_t cap_cols, int64_t *n_cols);
 /* htslib's per-column / per-read entry points on the device (tier T1 support; one column or one small batch per call):
  *   b200_errmod_cal   errmod_cal(em, n, m, bases, q) of htslib errmod.c (callers bam2bcf.c:121, phase.c:754, cut_target.c:84):
  *                     `bases` (q<<5|strand<<4|allele) is left sorted like the reference leaves it, q[m*m] receives the

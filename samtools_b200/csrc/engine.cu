@@ -252,6 +252,7 @@ __global__ void __launch_bounds__(TILE) k_mpileup_write(MpFmt fmt, const uint32_
 }
 #include "mpileup_ss.cuh"
 #include "mpileup_ent.cuh"
+#include "mpileup_cnt.cuh"
 
 struct DpFmt {
     View v; DpConf cf;
@@ -900,6 +901,39 @@ extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c,
     }
     CK(cudaEventRecord(e->ev1, e->stream));
     return text_end(e, e->col_off + nt, bound, out, out_cap, out_len);
+}
+
+extern "C" int b200_mpileup_counts(b200_engine_t *e, int32_t min_baseQ, uint32_t *out, size_t cap_cols, int64_t *n_cols)
+{
+    if (!e || !e->staged) { if (e) snprintf(e->err, sizeof e->err, "no staged batch"); return -1; }
+    if (e->sconf.mode != B200_MODE_MPILEUP) { snprintf(e->err, sizeof e->err, "mpileup counts need a batch staged in B200_MODE_MPILEUP"); return -1; }
+    CK(cudaSetDevice(e->device));
+    View v; fill_view(e, v, nullptr, nullptr, 0, 0, 1);
+    const int64_t n = v.ncols;
+    *n_cols = n; e->last_kernel_ms = 0;
+    if (out && cap_cols < (size_t)n) { snprintf(e->err, sizeof e->err, "count buffer too small: need %lld columns", (long long)n); return -2; }
+    if (n == 0) return 0;
+    // the kernel writes straight into a caller's device buffer; host memory gets the planes through the handle's buffer
+    uint32_t *dst = nullptr;
+    if (out) {
+        cudaPointerAttributes a;
+        CK(cudaPointerGetAttributes(&a, out));
+        if (a.type == cudaMemoryTypeDevice) {
+            if (a.device != e->device) { snprintf(e->err, sizeof e->err, "count buffer is on device %d, the handle on device %d", a.device, e->device); return -1; }
+            dst = out;
+        } else if (a.type == cudaMemoryTypeManaged) dst = out;
+    }
+    const size_t words = (size_t)e->n_files * CNT_PLANES * (size_t)n;
+    if (!dst) { ENSURE(cnt, words); dst = e->cnt; }
+    const int64_t warps = (int64_t)e->n_files * ((n + 31) / 32);
+    CK(cudaEventRecord(e->ev0, e->stream));
+    k_mp_counts<<<nblk(warps, CNT_WARPS), CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, (int32_t)((n + 31) / 32), dst); e->launches++;
+    CK(cudaEventRecord(e->ev1, e->stream));
+    if (out && dst != out) CK(cudaMemcpyAsync(out, dst, words * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaGetLastError());
+    float ms = 0; cudaEventElapsedTime(&ms, e->ev0, e->ev1); e->last_kernel_ms = ms;
+    return 0;
 }
 
 extern "C" int b200_depth_text(b200_engine_t *e, const b200_depth_conf_t *c, char *out, size_t out_cap, size_t *out_len)

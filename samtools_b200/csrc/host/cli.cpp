@@ -1,6 +1,7 @@
 // cli.cpp -- `b200samtools mpileup|depth|coverage|bedcov|gl`: the reference's CLI surface
-// for the pileup hot path, driving the CUDA engine through its C ABI; `index` writes the
-// BAI / CSI those commands read a region through.
+// for the pileup hot path, driving the CUDA engine through its C ABI; `counts` prints the
+// per-column base and indel counts of mpileup's rows; `index` writes the BAI / CSI those
+// commands read a region through.
 //
 // Option surfaces follow bam_plcmd.c:1096-1223 (mpileup), bam2depth.c:757-882
 // (depth) and coverage.c:343-424 (coverage), SURVEY.md Appendix B.  What stays
@@ -27,12 +28,17 @@
 #include <cstring>
 #include <cerrno>
 #include <algorithm>
+#include <charconv>
 #include <thread>
 #include <queue>
 #include <set>
 #include <unordered_map>
 
 using namespace b200;
+
+// The count output is an optional part of an engine build: the CLI links against any implementation of the C ABI (the CUDA
+// library, or a CPU debug build of the column code that may not provide it), and `counts` refuses to run on one without it.
+#pragma weak b200_mpileup_counts
 
 namespace {
 
@@ -124,6 +130,7 @@ std::vector<int> worker_devices()
 // One engine handle of a driver: its packer, record cursors (one per file) and the output of the window it last ran.
 struct WinWorker {
     Engine eng; PackedBatch pb; std::vector<char> out; std::vector<size_t> sel, cursor; size_t need = 0; int rc = 0; std::string err;
+    std::vector<uint32_t> cnt;   // count planes of the window (counts)
     void rewind() { std::fill(cursor.begin(), cursor.end(), 0); }
     int fail(const char *tool) { rc = -1; err = std::string("samtools ") + tool + ": " + b200_last_error(eng.e); return -1; }
 };
@@ -303,6 +310,7 @@ struct MpOpts {
     std::unique_ptr<Fasta> fa; std::unique_ptr<Bed> bed;
     std::set<std::string> rg_excl; bool have_rg = false;
     bool gl = false;
+    bool counts = false;   // `counts`: the rows of mpileup as per-column counts (b200_mpileup_counts)
     // host columns (bam_plcmd.c:727-855): record fields in the order of the MPLP_PRINT_* bits, then aux tags in the order given
     std::vector<std::string> xcols;      // "QNAME" "FLAG" "RNAME" "POS" "MAPQ" "RNEXT" "PNEXT" "RLEN" or a two-letter tag
     int n_xfields = 0;                   // how many of them are record fields (joined with ','; tags use x_sep)
@@ -512,6 +520,30 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn, const std::vector
                 }
                 return;
             }
+            if (o.counts) {
+                // one row per line mpileup prints: some file has a read over the column, or -a and the column is inside the
+                // contig; then the BED filter
+                int64_t n = 0; const size_t cap = (size_t)st.n_cols, plane = cap;
+                w.cnt.resize((size_t)nfn * B200_COUNT_PLANES * cap + 1);
+                if (b200_mpileup_counts(w.eng.e, o.min_baseQ, w.cnt.data(), cap, &n) != 0) { w.fail("counts"); return; }
+                const int64_t n_all = std::min(we, h.lens[(size_t)tid]) - wb;
+                for (int64_t c = 0; c < n; ++c) {
+                    bool any = false;
+                    for (int f = 0; f < nfn && !any; ++f) any = w.cnt[((size_t)f * B200_COUNT_PLANES + B200_COUNT_PLANES - 1) * plane + (size_t)c] > 0;
+                    if (!any && !(o.all && c < n_all)) continue;
+                    const int64_t p = wb + c;
+                    if (o.bed && !o.bed->overlap(name, p, p + 1)) continue;
+                    appendf(w, "%s\t%lld\t%c", name.c_str(), (long long)p + 1, (ref && p < (int64_t)ref->size()) ? (*ref)[(size_t)p] : 'N');
+                    const size_t need = w.need + (size_t)nfn * B200_COUNT_PLANES * 11 + 2;
+                    if (w.out.size() < need) w.out.resize(std::max(2 * w.out.size(), need));
+                    char *q = w.out.data() + w.need;
+                    for (int f = 0; f < nfn; ++f)
+                        for (int k = 0; k < B200_COUNT_PLANES; ++k) { *q++ = '\t'; q = std::to_chars(q, w.out.data() + w.out.size(), w.cnt[((size_t)f * B200_COUNT_PLANES + (size_t)k) * plane + (size_t)c]).ptr; }
+                    *q++ = '\n';
+                    w.need = (size_t)(q - w.out.data());
+                }
+                return;
+            }
             if (!o.xcols.empty() && render_host_columns(w) != 0) { w.fail("mpileup"); return; }
             const size_t bound = (size_t)b200_mpileup_text_bound(w.eng.e, &mc);
             if (w.out.size() < bound + 64) w.out.resize(bound + 64);
@@ -548,9 +580,13 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn, const std::vector
     return 0;
 }
 
-int main_mpileup(int argc, char **argv, bool gl)
+enum MpCmd { MP_TEXT, MP_GL, MP_COUNTS };
+// options of the pileup text that `counts` has no use for: -s -O -M, --output-*, --no-output-*, --reverse-del
+bool text_only_option(int c) { return c == 's' || c == 'O' || c == 'M' || (c >= 5 && c <= 14); }
+
+int main_mpileup(int argc, char **argv, MpCmd cmd)
 {
-    MpOpts o; o.gl = gl;
+    MpOpts o; o.gl = cmd == MP_GL; o.counts = cmd == MP_COUNTS;
     const char *file_list = nullptr; bool use_orphan = false, has_index_file = false;
     int want_fields = 0; std::vector<std::string> want_tags;
     static const struct option lo[] = {
@@ -568,6 +604,13 @@ int main_mpileup(int argc, char **argv, bool gl)
     int c;
     optind = 1;
     while ((c = getopt_long(argc, argv, "Af:r:l:q:Q:RC:Bd:b:o:EG:6OsxXaM", lo, nullptr)) >= 0) {
+        if (o.counts && text_only_option(c)) {
+            char opt[3] = {'-', (char)c, 0};
+            fprintf(stderr, "b200samtools counts: %s is an option of the pileup text\n\n"
+                            "Usage: b200samtools counts [-f ref.fa] [-r reg] [-l bed] [-b list] [-X] [-q INT] [-Q INT] [-B] [-E] [-C INT] [-d INT]\n"
+                            "                           [-x] [-A] [-6] [-G file] [-R] [--rf FLAGS] [--ff FLAGS] [-a[a]] [-o out] in1.bam [in2.bam ...]\n", c < 32 ? argv[optind - 1] : opt);
+            return 1;
+        }
         switch (c) {
         case 'x': o.overlaps = false; break;
         case 1: o.rf = parse_flag(optarg); if (o.rf < 0) { fprintf(stderr, "Could not parse --rf %s\n", optarg); return 1; } break;
@@ -627,6 +670,7 @@ int main_mpileup(int argc, char **argv, bool gl)
         default: fprintf(stderr, "\nUsage: samtools mpileup [options] in1.bam [in2.bam [...]]\n"); return 1;
         }
     }
+    if (o.counts && !b200_mpileup_counts) { fprintf(stderr, "b200samtools counts: this engine build has no count output\n"); return 1; }
     if (!o.realn && o.redo_baq) { fprintf(stderr, "Error: The -B option cannot be combined with -E\n"); return 1; }
     if (use_orphan) o.no_orphan = false;
     {   // record fields print in the order of the MPLP_PRINT_* bits (bam_plcmd.c:185-196,728-795), tags after them in the order given
@@ -1178,10 +1222,11 @@ int main_index(int argc, char **argv)
 
 int main(int argc, char **argv)
 {
-    if (argc < 2) { fprintf(stderr, "Usage: b200samtools <mpileup|depth|coverage|bedcov|gl|index> [options]\n"); return 1; }
+    if (argc < 2) { fprintf(stderr, "Usage: b200samtools <mpileup|depth|coverage|bedcov|gl|counts|index> [options]\n"); return 1; }
     std::string cmd = argv[1];
-    if (cmd == "mpileup") return main_mpileup(argc - 1, argv + 1, false);
-    if (cmd == "gl") return main_mpileup(argc - 1, argv + 1, true);
+    if (cmd == "mpileup") return main_mpileup(argc - 1, argv + 1, MP_TEXT);
+    if (cmd == "gl") return main_mpileup(argc - 1, argv + 1, MP_GL);
+    if (cmd == "counts") return main_mpileup(argc - 1, argv + 1, MP_COUNTS);
     if (cmd == "depth") return main_depth(argc - 1, argv + 1);
     if (cmd == "coverage") return main_coverage(argc - 1, argv + 1);
     if (cmd == "bedcov") return main_bedcov(argc - 1, argv + 1);

@@ -330,6 +330,22 @@ PLP_HD int ent_qual(const View &v, const ReadDesc &d, const Ent &e)
 }
 
 // ---- mpileup text for one (read, column) ------------------------------------
+// reference code of column c as pileup_seq compares it (bam_plcmd.c:74-80); 0x10 without a FASTA
+PLP_HD uint32_t ent_ref_code(const View &v, int32_t c)
+{
+    if (!v.ref) return 0x10u;
+    if ((int64_t)c < v.ref_len_rel) { const int64_t ri = (int64_t)c - v.ref_off; if (ri >= 0 && ri < v.ref_n) return (uint32_t)nt16_of((unsigned char)v.ref[ri]); }
+    return 15u;
+}
+
+// the base an entry that is not a deletion shows: the read's nt16 code, 0 ('.' / ',') where it equals the column's
+// reference code rb (ent_ref_code; bam_plcmd.c:74-80)
+PLP_HD int mp_base_code(int code, uint32_t rb) { return (uint32_t)code == rb ? 0 : code; }
+PLP_HD int mp_entry_base(const View &v, const ReadDesc &d, const Ent &e, int32_t c)
+{
+    return mp_base_code(e.qpos < d.l_qseq ? base4(v.seq4, d.qoff, e.qpos) : 15, ent_ref_code(v, c));
+}
+
 PLP_HD int mp_entry_size(const MpConf &cf, const ReadDesc &d, const uint32_t *cg, const Ent &e)
 {
     int sz = 1;
@@ -354,18 +370,8 @@ PLP_HD int mp_entry_write(const View &v, const MpConf &cf, const ReadDesc &d, co
     char *p0 = p;
     const bool rev = d.fl & RD_REV;
     if (!cf.no_ends && e.is_head) { *p++ = '^'; *p++ = (char)(d.mapq > 93 ? 126 : d.mapq + 33); }
-    if (!e.is_del) {
-        int ch = e.qpos < d.l_qseq ? base4(v.seq4, d.qoff, e.qpos) : 15;
-        if (v.ref) {
-            int rb = 15;
-            if ((int64_t)c < v.ref_len_rel) {
-                int64_t i = (int64_t)c - v.ref_off;
-                if (i >= 0 && i < v.ref_n) rb = nt16_of((unsigned char)v.ref[i]);
-            }
-            if (ch == rb) ch = 0;
-        }
-        *p++ = base_char(ch, rev);
-    } else *p++ = e.is_refskip ? (rev ? '<' : '>') : ((rev && cf.rev_del) ? '#' : '*');
+    if (!e.is_del) *p++ = base_char(mp_entry_base(v, d, e, c), rev);
+    else *p++ = e.is_refskip ? (rev ? '<' : '>') : ((rev && cf.rev_del) ? '#' : '*');
     int del_len = -e.indel;
     if (e.indel > 0) {
         int len = ins_scan(d, cg, e.k, del_len);
@@ -396,6 +402,29 @@ PLP_HD int mp_entry_write(const View &v, const MpConf &cf, const ReadDesc &d, co
     }
     if (!cf.no_ends && e.is_tail) *p++ = '$';
     return (int)(p - p0);
+}
+
+// ---- per-column counts of the entries (mpileup_cnt.cuh): what a parser of the "--reverse-del" text counts ----------
+// Planes per file: kinds 0-6 and the two indel events of forward-strand entries, the same for reverse-strand entries
+// (+ CNT_REV), then the reads over the column before -Q.
+enum { CNT_A = 0, CNT_C, CNT_G, CNT_T, CNT_N, CNT_DEL, CNT_SKIP, CNT_INS_NEXT, CNT_DEL_NEXT, CNT_REV = 9, CNT_NPLP = 18, CNT_PLANES = B200_COUNT_PLANES };
+// channel of a reference character: A C G T in either case -> 0..3, anything else -> N
+PLP_HD int ref_chan(char ch)
+{
+    switch (up(ch)) { case 'A': return CNT_A; case 'C': return CNT_C; case 'G': return CNT_G; case 'T': return CNT_T; default: return CNT_N; }
+}
+// the entry of read d at column c (cursor e), as counts: bits 0-3 its kind (CNT_A .. CNT_SKIP), bit 4 a "+n" follows, bit 5
+// a "-n" follows -- what mp_entry_write prints for it.  The caller applies -Q first: a failing entry prints nothing.
+enum { CNT_BIT_INS = 16, CNT_BIT_DEL = 32 };
+PLP_HD int mp_entry_channel(const View &v, const ReadDesc &d, const uint32_t *cg, const Ent &e, int32_t c)
+{
+    int x;
+    if (e.is_del) x = e.is_refskip ? CNT_SKIP : CNT_DEL;
+    else { const int ch = mp_entry_base(v, d, e, c); x = ch ? nt16_int_of(ch) : ref_chan(ref_char(v, c)); }
+    int del_len = -e.indel;
+    if (e.indel > 0) { ins_scan(d, cg, e.k, del_len); x |= CNT_BIT_INS; }
+    if (del_len > 0) x |= CNT_BIT_DEL;
+    return x;
 }
 
 // per (column, file) sizes
@@ -550,12 +579,7 @@ PLP_HD char *mp_file_write(const View &v, const MpConf &cf, int f, int tile, int
         if (cf.out_qpos5) *pb5++ = '\t';
         const ReadRange rr = read_range(v, f, tile);
         int n = 0;
-        // reference base of this column, once (bam_plcmd.c:74-80)
-        int rb = -1;
-        if (v.ref) {
-            rb = 15;
-            if ((int64_t)c < v.ref_len_rel) { const int64_t ri = (int64_t)c - v.ref_off; if (ri >= 0 && ri < v.ref_n) rb = nt16_of((unsigned char)v.ref[ri]); }
-        }
+        const uint32_t rb = ent_ref_code(v, c);   // reference base of this column, once
         const bool ends = !cf.no_ends, extras = (cf.out_mapq | cf.out_qpos | cf.out_qpos5) != 0;
         const int minq = cf.min_baseQ;
         // Descriptors travel through the loop as four raw words (rpos, rend, qoff, qstart | mapq << 16 | flags << 24):
@@ -597,9 +621,7 @@ PLP_HD char *mp_file_write(const View &v, const MpConf &cf, int f, int tile, int
                 const bool rev = (r.pk & kRev) != 0;
                 const uint32_t par = (r.qoff ^ r.pk ^ rel) & 1u;          // parity of the query index qoff + qstart + rel
                 if (ends && rel == 0) { *ps++ = '^'; *ps++ = (char)(mapq > 93 ? 126 : mapq + 33); }
-                int ch = (int)((pre.sb >> ((par ^ 1u) << 2)) & 0xfu);
-                if (ch == rb) ch = 0;
-                *ps++ = base_char(ch, rev);
+                *ps++ = base_char(mp_base_code((int)((pre.sb >> ((par ^ 1u) << 2)) & 0xfu), rb), rev);
                 if (ends && c == r.rend - 1) *ps++ = '$';
                 if (extras) {
                     const int32_t qpos = (int32_t)(r.pk & 0xffffu) + (int32_t)rel;
@@ -725,20 +747,12 @@ PLP_HD uint32_t umin32(uint32_t a, uint32_t b)
 #endif
 }
 
-// reference code of column c as pileup_seq compares it (bam_plcmd.c:74-80); 0x10 without a FASTA
-PLP_HD uint32_t ent_ref_code(const View &v, int32_t c)
-{
-    if (!v.ref) return 0x10u;
-    if ((int64_t)c < v.ref_len_rel) { const int64_t ri = (int64_t)c - v.ref_off; if (ri >= 0 && ri < v.ref_n) return (uint32_t)nt16_of((unsigned char)v.ref[ri]); }
-    return 15u;
-}
-
 // entry of one aligned base: q quality byte, code 4-bit base, rb reference code of the column (0x10: none),
 // tab = ".ACMGRSVTWYHKDBN,acmgrsvtwyhkdbn" (forward strand, then reverse), flags = 0x80 (head) | 0x8000 (tail)
 PLP_HD uint32_t ent_plain(uint32_t q, uint32_t code, uint32_t rb, uint32_t rev, int minq, uint32_t flags, const uint8_t *tab)
 {
     if ((int)q < minq) return 0;
-    if (code == rb) code = 0;
+    code = (uint32_t)mp_base_code((int)code, rb);
     return (uint32_t)tab[rev * 16u + code] | umin32(q + 33u, 126u) << 8 | flags;
 }
 
@@ -818,11 +832,8 @@ PLP_HD uint32_t ent_generic(const View &v, const MpConf &cf, const ReadDesc &d, 
     if (e.indel != 0) return ENT_SPECIAL;
     const uint32_t rev = (d.fl & RD_REV) ? 1u : 0u;
     uint32_t ch;
-    if (!e.is_del) {
-        uint32_t code = e.qpos < d.l_qseq ? (uint32_t)base4(v.seq4, d.qoff, e.qpos) : 15u;
-        if (code == rb) code = 0;
-        ch = tab[rev * 16u + code];
-    } else ch = (uint32_t)(e.is_refskip ? (rev ? '<' : '>') : ((rev && cf.rev_del) ? '#' : '*'));
+    if (!e.is_del) ch = tab[rev * 16u + (uint32_t)mp_base_code(e.qpos < d.l_qseq ? base4(v.seq4, d.qoff, e.qpos) : 15, rb)];
+    else ch = (uint32_t)(e.is_refskip ? (rev ? '<' : '>') : ((rev && cf.rev_del) ? '#' : '*'));
     uint32_t x = ch | umin32((uint32_t)q + 33u, 126u) << 8;
     if (!cf.no_ends) x |= (e.is_head ? 0x80u : 0u) | (e.is_tail ? 0x8000u : 0u);
     return x;

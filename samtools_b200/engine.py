@@ -20,7 +20,9 @@ EXPORTS = ['b200_engine_create', 'b200_engine_destroy', 'b200_last_error', 'b200
            'b200_mpileup_text', 'b200_depth_text', 'b200_coverage', 'b200_coverage_hist', 'b200_glf', 'b200_fetch_qual',
            'b200_fetch_mapq_keep', 'b200_pileup_entries', 'b200_last_kernel_ms', 'b200_last_stage_ms', 'b200_set_keep_raw', 'b200_restage', 'b200_last_stage_device_ms',
            'b200_launch_count', 'b200_last_mpileup_parts_ms', 'b200_gl_rng_draws', 'b200_last_baq_ms',
-           'b200_errmod_cal', 'b200_glfgen', 'b200_cap_mapq', 'b200_mpileup_text_bound', 'b200_depth_text_bound', 'b200_bedcov']
+           'b200_errmod_cal', 'b200_glfgen', 'b200_cap_mapq', 'b200_mpileup_text_bound', 'b200_depth_text_bound', 'b200_bedcov',
+           'b200_mpileup_counts']
+COUNT_PLANES = 19   # b200_mpileup_counts: per file A C G T N del skip +ins -del, forward then reverse strand, then n_plp
 
 
 class Batch(C.Structure):
@@ -89,6 +91,7 @@ def load_library():
         lib.b200_depth_text.argtypes = [C.c_void_p, C.POINTER(DepthConf), C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
         lib.b200_coverage.argtypes = [C.c_void_p, C.POINTER(CoverageConf), C.POINTER(CoverageSums)]
         lib.b200_glf.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
+        lib.b200_mpileup_counts.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64)]
         lib.b200_fetch_qual.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_fetch_mapq_keep.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_pileup_entries.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -136,7 +139,9 @@ class Engine:
         if self.lib.b200_engine_create(device, C.byref(h)) != 0:
             raise RuntimeError('b200_engine_create failed: no usable CUDA device (the engine has no CPU fallback)')
         self.h = h
+        self.device = device
         self._keep = None
+        self._n_files = self._n_cols = 0
 
     def close(self):
         if self.h:
@@ -170,8 +175,10 @@ class Engine:
         b.ref_len = 0 if ref is None else int(soa.get('ref_len', len(ref)))
         st = StageStats()
         self._keep = (soa, name)
+        self._n_files = b.n_files
         if self.lib.b200_stage(self.h, C.byref(b), C.byref(conf), C.byref(st)) != 0:
             self._err('b200_stage')
+        self._n_cols = st.n_cols
         return st
 
     def set_keep_raw(self, on=True):
@@ -183,6 +190,7 @@ class Engine:
         st = StageStats()
         if self.lib.b200_restage(self.h, C.byref(st)) != 0:
             self._err('b200_restage')
+        self._n_cols = st.n_cols
         return st
 
     def _text(self, fn, conf, out=None, fetch=True):
@@ -228,6 +236,27 @@ class Engine:
             self._err('b200_glf')
         k = n.value
         return pos[:k], nb[:k * n_files].reshape(k, n_files), qs[:k * n_files * 4].reshape(k, n_files, 4), p25[:k * n_files * 25].reshape(k, n_files, 25)
+
+    def mpileup_counts(self, min_baseQ=13, out=None):
+        """Per-column strand-split base and indel counts of the staged window (b200_mpileup_counts): a numpy uint32
+        [n_files, 19, n] array, or, given `out`, a contiguous torch.int32 CUDA tensor of that shape on the handle's device,
+        filled in place on the device (and returned)."""
+        n = C.c_int64(0)
+        shape = (self._n_files, COUNT_PLANES, self._n_cols)     # the stage's n_cols are the columns of the planes
+        if out is None:
+            a = np.zeros(shape, np.uint32)
+            if self.lib.b200_mpileup_counts(self.h, min_baseQ, _ptr(a), shape[2], C.byref(n)) != 0:
+                self._err('b200_mpileup_counts')
+            return a
+        import torch
+        if out.dtype != torch.int32 or not out.is_cuda or not out.is_contiguous() or out.device.index != self.device:
+            raise ValueError(f'out must be a contiguous torch.int32 tensor on cuda:{self.device}')
+        if tuple(out.shape) != shape:
+            raise ValueError(f'out must have shape {list(shape)}')
+        torch.cuda.current_stream(out.device).synchronize()   # the engine writes on its own stream
+        if self.lib.b200_mpileup_counts(self.h, min_baseQ, C.c_void_p(out.data_ptr()), shape[2], C.byref(n)) != 0:
+            self._err('b200_mpileup_counts')
+        return out
 
     def fetch_qual(self, nbytes):
         q = np.zeros(nbytes, np.uint8)
