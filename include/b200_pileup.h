@@ -25,6 +25,7 @@
  *   b200_bedcov()         per-interval column reducers    bedcov.c:303-331
  *   b200_glf()            bcf_call_glfgen + errmod_cal    bam2bcf.c:65-123 (+ htslib errmod.c)
  *   b200_mpileup_counts() pileup_seq, as numbers           bam_plcmd.c:54-169 -> per-column strand-split base / indel counts
+ *   b200_mpileup_indels() pileup_seq's +n / -n tokens      bam_plcmd.c:54-169 -> per-column indel alleles, strand-split support
  *   b200_pileup_entries() bam_plp64_next/resolve_cigar2   (htslib sam.c) -> arrays of bam_pileup1_t fields
  *
  * Conventions: plain C, caller-owned host buffers, int return codes (0 ok,
@@ -233,6 +234,26 @@ int b200_glf(b200_engine_t *e, int32_t min_baseQ, int64_t *n_cols, int64_t *col_
  * cap_cols < n returns -2.  *n_cols always receives n.  Needs a batch staged in B200_MODE_MPILEUP. */
 #define B200_COUNT_PLANES 19
 int b200_mpileup_counts(b200_engine_t *e, int32_t min_baseQ, uint32_t *out, size_t cap_cols, int64_t *n_cols);
+/* per-column indel alleles of the mpileup column stage: the distinct "+n..." / "-n" tokens that the `mpileup` text of the
+ * staged window prints after the entries passing -Q (min_baseQ), one row per (column, file, allele), ordered by column
+ * c = position - window start, then file, then first appearance in the line (file order of the reads; a read's insertion
+ * before its deletion).  len >= 0: an insertion of len symbols, seq[seq_off, seq_off + len) -- the read's upper-case IUPAC
+ * bases, 'N' past the read's sequence, '*' for a pad; len < 0: a deletion of -len reference bases (named by its length:
+ * the bases are the reference's at c+1 .. c-len).  fwd / rev: the entries on each strand that carry the token.  Per
+ * (column, file) the fwd sums over insertions and deletions are planes 7 and 8 of b200_mpileup_counts, the rev sums 16 and
+ * 17.  32 bytes per row (an int32 [n, 8] view).
+ *   b200_mpileup_indels  computes the table and keeps it in HBM; *n_alleles and *n_seq_bytes receive its size.  Needs a batch
+ *                        staged in B200_MODE_MPILEUP.  b200_last_kernel_ms() covers it.
+ *   b200_fetch_indels    copies the table of the last b200_mpileup_indels since the batch was staged to host or device memory
+ *                        (a device buffer must be on the handle's device); either pointer may be NULL to skip its part.
+ *                        cap_alleles < n_alleles or cap_seq < n_seq_bytes returns -2. */
+typedef struct {
+    int32_t col, file, len;
+    uint32_t fwd, rev, pad;
+    uint64_t seq_off;
+} b200_indel_t;
+int b200_mpileup_indels(b200_engine_t *e, int32_t min_baseQ, int64_t *n_alleles, uint64_t *n_seq_bytes);
+int b200_fetch_indels(b200_engine_t *e, b200_indel_t *alleles, size_t cap_alleles, char *seq, size_t cap_seq);
 /* htslib's per-column / per-read entry points on the device (tier T1 support; one column or one small batch per call):
  *   b200_errmod_cal   errmod_cal(em, n, m, bases, q) of htslib errmod.c (callers bam2bcf.c:121, phase.c:754, cut_target.c:84):
  *                     `bases` (q<<5|strand<<4|allele) is left sorted like the reference leaves it, q[m*m] receives the

@@ -253,6 +253,7 @@ __global__ void __launch_bounds__(TILE) k_mpileup_write(MpFmt fmt, const uint32_
 #include "mpileup_ss.cuh"
 #include "mpileup_ent.cuh"
 #include "mpileup_cnt.cuh"
+#include "mpileup_indel.cuh"
 
 struct DpFmt {
     View v; DpConf cf;
@@ -595,6 +596,7 @@ extern "C" int b200_stage(b200_engine_t *e, const b200_batch_t *b, const b200_st
 // mate-overlap tweak.  Works on the arrays resident in device memory (b200_stage uploads them first).
 static int stage_device(b200_engine *e, b200_stage_stats_t *stats)
 {
+    e->ind_ready = false;   // the indel table belongs to the batch it was computed on
     const int64_t n = e->n;
     const b200_stage_conf_t *cf = &e->sconf;
     if (e->keep_raw && n > 0) {
@@ -933,6 +935,107 @@ extern "C" int b200_mpileup_counts(b200_engine_t *e, int32_t min_baseQ, uint32_t
     CK(cudaStreamSynchronize(e->stream));
     CK(cudaGetLastError());
     float ms = 0; cudaEventElapsedTime(&ms, e->ev0, e->ev1); e->last_kernel_ms = ms;
+    return 0;
+}
+
+// Test knob: B200_INDEL_KEY_BITS=k keeps the low k bits of every allele key, so different insertions share keys and the
+// table has to tell them apart by their bytes.
+static uint64_t indel_key_mask()
+{
+    const char *s = getenv("B200_INDEL_KEY_BITS");
+    const int b = s ? atoi(s) : 64;
+    return b >= 64 ? ~0ull : b <= 0 ? 0ull : (1ull << b) - 1;
+}
+
+extern "C" int b200_mpileup_indels(b200_engine_t *e, int32_t min_baseQ, int64_t *n_alleles, uint64_t *n_seq_bytes)
+{
+    if (!e || !e->staged) { if (e) snprintf(e->err, sizeof e->err, "no staged batch"); return -1; }
+    if (e->sconf.mode != B200_MODE_MPILEUP) { snprintf(e->err, sizeof e->err, "mpileup indels need a batch staged in B200_MODE_MPILEUP"); return -1; }
+    CK(cudaSetDevice(e->device));
+    e->ind_ready = false; e->ind_n = 0; e->ind_nseq = 0; e->last_kernel_ms = 0;
+    *n_alleles = 0; *n_seq_bytes = 0;
+    View v; fill_view(e, v, nullptr, nullptr, 0, 0, 1);
+    const int64_t n = v.ncols, segs = n * e->n_files;
+    // bounds from the stage's sum over the kept reads of 3 + (12 + length) per I, P and D op: an event follows a distinct I /
+    // P / D op of its read, and its symbols are the lengths of the I / P ops after the entry
+    const uint64_t ops = e->sum_indel_text - 3ull * (uint64_t)e->acc_n_kept;
+    const uint64_t cap64 = ops / 12 + 1, sym_cap = ops + 1;
+    if (segs + 2 > INT32_MAX || cap64 > (uint64_t)INT32_MAX / 2) { snprintf(e->err, sizeof e->err, "window too large for the indel table"); return -1; }
+    const uint32_t cap = (uint32_t)cap64;
+    if (n == 0) { e->ind_ready = true; return 0; }
+    ENSURE(ind_cnt, (size_t)segs + 1); ENSURE(ind_off, (size_t)segs + 2);
+    ENSURE(ind_ev, (size_t)cap * sizeof(IndelEv)); ENSURE(ind_len, (size_t)cap + 1); ENSURE(ind_soff, (size_t)cap + 2);
+    ENSURE(ind_key, cap); ENSURE(ind_slot, cap); ENSURE(ind_first, (size_t)cap + 1); ENSURE(ind_bytes, (size_t)cap + 1);
+    ENSURE(ind_aidx, (size_t)cap + 2); ENSURE(ind_aseq, (size_t)cap + 2); ENSURE(ind_tbl, 2 * (size_t)cap); ENSURE(ind_tcnt, 4 * (size_t)cap);
+    ENSURE(ind_sym, sym_cap); ENSURE(ind_tab, cap); ENSURE(ind_seq, sym_cap);
+    IndelEv *ev = (IndelEv *)e->ind_ev;
+    const int32_t n_groups = (int32_t)((n + 31) / 32);
+    const int wb = nblk((int64_t)e->n_files * n_groups, IND_WARPS), eb = nblk(cap, 256);
+    const uint32_t *n_ev = e->ind_off + segs;
+    CK(cudaEventRecord(e->ev0, e->stream));
+    k_ind_walk<false><<<wb, IND_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, e->ind_cnt, nullptr, nullptr, nullptr, 0); e->launches++;
+    if (launch_scan<ScanSum, 4, false>(e, e->ind_cnt, e->ind_off, segs)) return -1;
+    CK(cudaMemsetAsync(e->ind_len, 0, (size_t)cap * 4, e->stream));
+    k_ind_walk<true><<<wb, IND_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, nullptr, e->ind_off, ev, e->ind_len, cap); e->launches++;
+    if (launch_scan<ScanSum, 4, false>(e, e->ind_len, e->ind_soff, cap)) return -1;
+    k_ind_syms<<<eb, 256, 0, e->stream>>>(v, ev, n_ev, cap, e->ind_soff, sym_cap, e->ind_sym, indel_key_mask(), e->ind_key); e->launches++;
+    CK(cudaMemsetAsync(e->ind_tbl, 0xff, 2 * (size_t)cap * 4, e->stream));
+    CK(cudaMemsetAsync(e->ind_tcnt, 0, 4 * (size_t)cap * 4, e->stream));
+    k_ind_insert<<<eb, 256, 0, e->stream>>>(ev, n_ev, cap, e->ind_key, e->ind_soff, e->ind_sym, e->ind_tbl, e->ind_tcnt, e->ind_slot); e->launches++;
+    k_ind_mark<<<eb, 256, 0, e->stream>>>(ev, n_ev, cap, e->ind_tbl, e->ind_slot, e->ind_first, e->ind_bytes); e->launches++;
+    if (launch_scan<ScanSum, 4, false>(e, e->ind_first, e->ind_aidx, cap)) return -1;
+    if (launch_scan<ScanSum, 4, false>(e, e->ind_bytes, e->ind_aseq, cap)) return -1;
+    k_ind_emit<<<eb, 256, 0, e->stream>>>(ev, n_ev, cap, e->ind_tcnt, e->ind_slot, e->ind_first, e->ind_aidx, e->ind_aseq, e->ind_soff,
+                                          e->ind_sym, e->ind_tab, e->ind_seq); e->launches++;
+    CK(cudaEventRecord(e->ev1, e->stream));
+    uint32_t h_ev = 0, h_n = 0; uint64_t h_sym = 0, h_seq = 0;
+    CK(cudaMemcpyAsync(&h_ev, n_ev, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(&h_sym, e->ind_soff + cap, 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(&h_n, e->ind_aidx + cap, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(&h_seq, e->ind_aseq + cap, 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaGetLastError());
+    if (h_ev > cap || h_sym > sym_cap) {
+        snprintf(e->err, sizeof e->err, "internal: %u indel events / %llu symbols exceed the stage's bound %u / %llu", h_ev,
+                 (unsigned long long)h_sym, cap, (unsigned long long)sym_cap);
+        return -1;
+    }
+    float ms = 0; cudaEventElapsedTime(&ms, e->ev0, e->ev1); e->last_kernel_ms = ms;
+    e->ind_n = h_n; e->ind_nseq = h_seq; e->ind_ready = true;
+    *n_alleles = h_n; *n_seq_bytes = h_seq;
+    return 0;
+}
+
+// cudaMemcpyDefault destination check: a device buffer must be on the handle's device
+static int check_dst(b200_engine *e, const void *p, const char *what)
+{
+    cudaPointerAttributes a;
+    CK(cudaPointerGetAttributes(&a, p));
+    if (a.type == cudaMemoryTypeDevice && a.device != e->device) {
+        snprintf(e->err, sizeof e->err, "%s buffer is on device %d, the handle on device %d", what, a.device, e->device);
+        return -1;
+    }
+    return 0;
+}
+
+extern "C" int b200_fetch_indels(b200_engine_t *e, b200_indel_t *alleles, size_t cap_alleles, char *seq, size_t cap_seq)
+{
+    if (!e || !e->staged || !e->ind_ready) {
+        if (e) snprintf(e->err, sizeof e->err, "no indel table: call b200_mpileup_indels on the staged batch first");
+        return -1;
+    }
+    CK(cudaSetDevice(e->device));
+    if (alleles && cap_alleles < (size_t)e->ind_n) { snprintf(e->err, sizeof e->err, "allele buffer too small: need %lld rows", (long long)e->ind_n); return -2; }
+    if (seq && cap_seq < e->ind_nseq) { snprintf(e->err, sizeof e->err, "symbol buffer too small: need %llu bytes", (unsigned long long)e->ind_nseq); return -2; }
+    if (alleles && e->ind_n) {
+        if (check_dst(e, alleles, "allele")) return -1;
+        CK(cudaMemcpyAsync(alleles, e->ind_tab, (size_t)e->ind_n * sizeof(b200_indel_t), cudaMemcpyDefault, e->stream));
+    }
+    if (seq && e->ind_nseq) {
+        if (check_dst(e, seq, "symbol")) return -1;
+        CK(cudaMemcpyAsync(seq, e->ind_seq, e->ind_nseq, cudaMemcpyDefault, e->stream));
+    }
+    CK(cudaStreamSynchronize(e->stream));
     return 0;
 }
 

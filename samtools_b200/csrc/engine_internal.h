@@ -43,6 +43,13 @@ struct b200_engine {
     DBUF(int32_t, clip); DBUF(int64_t, next); DBUF(int32_t, cig_x); DBUF(int32_t, cig_y);
     DBUF(double, baq_f); DBUF(int32_t, baq_idx); DBUF(uint8_t, ref_codes); DBUF(uint16_t, ent); DBUF(uint16_t, ent2); DBUF(uint32_t, x_off); DBUF(char, x_dat); DBUF(int32_t, ov_pairs);
     DBUF(float, gl_out); DBUF(int32_t, gl_n); DBUF(uint32_t, gl_flag); DBUF(uint32_t, cnt);   // cnt: count planes of b200_mpileup_counts
+    // b200_mpileup_indels (mpileup_indel.cuh): per (column, file) event counts and offsets; per event the record (IndelEv),
+    // symbol count, symbol offset, key, table slot, first-appearance flag and allele bytes, allele index and allele symbol
+    // offset; 2 hash slots per event and their strand counts; the symbols of the events, then the table and its symbols
+    DBUF(uint32_t, ind_cnt); DBUF(uint32_t, ind_off); DBUF(uint8_t, ind_ev); DBUF(uint32_t, ind_len); DBUF(uint64_t, ind_soff);
+    DBUF(uint64_t, ind_key); DBUF(uint32_t, ind_slot); DBUF(uint32_t, ind_first); DBUF(uint32_t, ind_bytes); DBUF(uint32_t, ind_aidx);
+    DBUF(uint64_t, ind_aseq); DBUF(int32_t, ind_tbl); DBUF(uint32_t, ind_tcnt); DBUF(char, ind_sym); DBUF(b200_indel_t, ind_tab); DBUF(char, ind_seq);
+    bool ind_ready = false; int64_t ind_n = 0; uint64_t ind_nseq = 0;   // the table of the staged batch: rows, symbol bytes
     void *d_acc = nullptr;
     unsigned long long *d_misc = nullptr;   // 64 words of small device results; slots MISC_* below, each zeroed by its writer's caller
     double *d_beta = nullptr, *d_fk = nullptr, *d_lhet = nullptr;   // errmod tables
@@ -68,7 +75,9 @@ struct b200_engine {
     {
         void *ps[] = { qual0, mapq0, pos, flag, mapq, l_qseq, n_cigar, cigar_off, qual_off, mtid, mpos, isize, prev, rbits, cigar, seq4, qual,
                        ref, dname, file_start, state, rlen, desc, endv, pmax, glo, ghi, status, out, bed_beg, bed_end, col_n,
-                       col_off, col_state, tile_total, ovf_cnt, ovf_off, ovf_idx, ss_diff, ss_nplp, ss_fail, ss_extra, ents, clip, next, cig_x, cig_y, baq_f, baq_idx, ref_codes, ent, ent2, x_off, x_dat, ov_pairs, gl_out, gl_n, gl_flag, cnt, d_beta, d_fk, d_lhet, d_q2p, d_qthr };
+                       col_off, col_state, tile_total, ovf_cnt, ovf_off, ovf_idx, ss_diff, ss_nplp, ss_fail, ss_extra, ents, clip, next, cig_x, cig_y, baq_f, baq_idx, ref_codes, ent, ent2, x_off, x_dat, ov_pairs, gl_out, gl_n, gl_flag, cnt,
+                       ind_cnt, ind_off, ind_ev, ind_len, ind_soff, ind_key, ind_slot, ind_first, ind_bytes, ind_aidx, ind_aseq, ind_tbl, ind_tcnt,
+                       ind_sym, ind_tab, ind_seq, d_beta, d_fk, d_lhet, d_q2p, d_qthr };
         for (void *p : ps) if (p) cudaFree(p);
     }
 };

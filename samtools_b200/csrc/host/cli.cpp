@@ -1,7 +1,7 @@
 // cli.cpp -- `b200samtools mpileup|depth|coverage|bedcov|gl`: the reference's CLI surface
 // for the pileup hot path, driving the CUDA engine through its C ABI; `counts` prints the
-// per-column base and indel counts of mpileup's rows; `index` writes the BAI / CSI those
-// commands read a region through.
+// per-column base and indel counts of mpileup's rows, `indels` the indel alleles of its
+// columns; `index` writes the BAI / CSI those commands read a region through.
 //
 // Option surfaces follow bam_plcmd.c:1096-1223 (mpileup), bam2depth.c:757-882
 // (depth) and coverage.c:343-424 (coverage), SURVEY.md Appendix B.  What stays
@@ -36,9 +36,12 @@
 
 using namespace b200;
 
-// The count output is an optional part of an engine build: the CLI links against any implementation of the C ABI (the CUDA
-// library, or a CPU debug build of the column code that may not provide it), and `counts` refuses to run on one without it.
+// The count and indel outputs are optional parts of an engine build: the CLI links against any implementation of the C ABI
+// (the CUDA library, or a CPU debug build of the column code that may not provide them), and `counts` / `indels` refuse to run
+// on one without theirs.
 #pragma weak b200_mpileup_counts
+#pragma weak b200_mpileup_indels
+#pragma weak b200_fetch_indels
 
 namespace {
 
@@ -131,6 +134,7 @@ std::vector<int> worker_devices()
 struct WinWorker {
     Engine eng; PackedBatch pb; std::vector<char> out; std::vector<size_t> sel, cursor; size_t need = 0; int rc = 0; std::string err;
     std::vector<uint32_t> cnt;   // count planes of the window (counts)
+    std::vector<b200_indel_t> ind; std::string ind_seq;   // indel table of the window (indels)
     void rewind() { std::fill(cursor.begin(), cursor.end(), 0); }
     int fail(const char *tool) { rc = -1; err = std::string("samtools ") + tool + ": " + b200_last_error(eng.e); return -1; }
 };
@@ -311,6 +315,7 @@ struct MpOpts {
     std::set<std::string> rg_excl; bool have_rg = false;
     bool gl = false;
     bool counts = false;   // `counts`: the rows of mpileup as per-column counts (b200_mpileup_counts)
+    bool indels = false;   // `indels`: the indel alleles of mpileup's columns (b200_mpileup_indels)
     // host columns (bam_plcmd.c:727-855): record fields in the order of the MPLP_PRINT_* bits, then aux tags in the order given
     std::vector<std::string> xcols;      // "QNAME" "FLAG" "RNAME" "POS" "MAPQ" "RNEXT" "PNEXT" "RLEN" or a two-letter tag
     int n_xfields = 0;                   // how many of them are record fields (joined with ','; tags use x_sep)
@@ -544,6 +549,30 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn, const std::vector
                 }
                 return;
             }
+            if (o.indels) {
+                // one row per allele: chr pos ref file token fwd rev; a deletion's bases are the reference's (upper case, 'N'
+                // without a FASTA or past the contig: bam_plcmd.c:158)
+                int64_t na = 0; uint64_t ns = 0;
+                if (b200_mpileup_indels(w.eng.e, o.min_baseQ, &na, &ns) != 0) { w.fail("indels"); return; }
+                w.ind.resize((size_t)na + 1); w.ind_seq.resize(ns + 1);
+                if (b200_fetch_indels(w.eng.e, w.ind.data(), w.ind.size(), &w.ind_seq[0], w.ind_seq.size()) != 0) { w.fail("indels"); return; }
+                std::string tok;
+                for (int64_t k = 0; k < na; ++k) {
+                    const b200_indel_t &a = w.ind[(size_t)k];
+                    const int64_t p = wb + a.col;
+                    if (o.bed && !o.bed->overlap(name, p, p + 1)) continue;
+                    tok.assign(1, a.len >= 0 ? '+' : '-');
+                    tok += std::to_string(a.len >= 0 ? a.len : -a.len);
+                    if (a.len >= 0) tok.append(w.ind_seq, (size_t)a.seq_off, (size_t)a.len);
+                    else for (int64_t j = 1; j <= -(int64_t)a.len; ++j) {
+                        const char b = (ref && p + j < (int64_t)ref->size()) ? (*ref)[(size_t)(p + j)] : 'N';
+                        tok += (b >= 'a' && b <= 'z') ? (char)(b - 32) : b;
+                    }
+                    appendf(w, "%s\t%lld\t%c\t%d\t%s\t%u\t%u\n", name.c_str(), (long long)p + 1,
+                            (ref && p < (int64_t)ref->size()) ? (*ref)[(size_t)p] : 'N', a.file, tok.c_str(), a.fwd, a.rev);
+                }
+                return;
+            }
             if (!o.xcols.empty() && render_host_columns(w) != 0) { w.fail("mpileup"); return; }
             const size_t bound = (size_t)b200_mpileup_text_bound(w.eng.e, &mc);
             if (w.out.size() < bound + 64) w.out.resize(bound + 64);
@@ -580,13 +609,14 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn, const std::vector
     return 0;
 }
 
-enum MpCmd { MP_TEXT, MP_GL, MP_COUNTS };
-// options of the pileup text that `counts` has no use for: -s -O -M, --output-*, --no-output-*, --reverse-del
+enum MpCmd { MP_TEXT, MP_GL, MP_COUNTS, MP_INDELS };
+// options of the pileup text that `counts` and `indels` have no use for: -s -O -M, --output-*, --no-output-*, --reverse-del
 bool text_only_option(int c) { return c == 's' || c == 'O' || c == 'M' || (c >= 5 && c <= 14); }
 
 int main_mpileup(int argc, char **argv, MpCmd cmd)
 {
-    MpOpts o; o.gl = cmd == MP_GL; o.counts = cmd == MP_COUNTS;
+    MpOpts o; o.gl = cmd == MP_GL; o.counts = cmd == MP_COUNTS; o.indels = cmd == MP_INDELS;
+    const char *tool = o.indels ? "indels" : "counts";
     const char *file_list = nullptr; bool use_orphan = false, has_index_file = false;
     int want_fields = 0; std::vector<std::string> want_tags;
     static const struct option lo[] = {
@@ -604,11 +634,12 @@ int main_mpileup(int argc, char **argv, MpCmd cmd)
     int c;
     optind = 1;
     while ((c = getopt_long(argc, argv, "Af:r:l:q:Q:RC:Bd:b:o:EG:6OsxXaM", lo, nullptr)) >= 0) {
-        if (o.counts && text_only_option(c)) {
+        if ((o.counts || o.indels) && text_only_option(c)) {
             char opt[3] = {'-', (char)c, 0};
-            fprintf(stderr, "b200samtools counts: %s is an option of the pileup text\n\n"
-                            "Usage: b200samtools counts [-f ref.fa] [-r reg] [-l bed] [-b list] [-X] [-q INT] [-Q INT] [-B] [-E] [-C INT] [-d INT]\n"
-                            "                           [-x] [-A] [-6] [-G file] [-R] [--rf FLAGS] [--ff FLAGS] [-a[a]] [-o out] in1.bam [in2.bam ...]\n", c < 32 ? argv[optind - 1] : opt);
+            fprintf(stderr, "b200samtools %s: %s is an option of the pileup text\n\n"
+                            "Usage: b200samtools %s [-f ref.fa] [-r reg] [-l bed] [-b list] [-X] [-q INT] [-Q INT] [-B] [-E] [-C INT] [-d INT]\n"
+                            "                           [-x] [-A] [-6] [-G file] [-R] [--rf FLAGS] [--ff FLAGS] [-a[a]] [-o out] in1.bam [in2.bam ...]\n",
+                    tool, c < 32 ? argv[optind - 1] : opt, tool);
             return 1;
         }
         switch (c) {
@@ -671,6 +702,7 @@ int main_mpileup(int argc, char **argv, MpCmd cmd)
         }
     }
     if (o.counts && !b200_mpileup_counts) { fprintf(stderr, "b200samtools counts: this engine build has no count output\n"); return 1; }
+    if (o.indels && (!b200_mpileup_indels || !b200_fetch_indels)) { fprintf(stderr, "b200samtools indels: this engine build has no indel output\n"); return 1; }
     if (!o.realn && o.redo_baq) { fprintf(stderr, "Error: The -B option cannot be combined with -E\n"); return 1; }
     if (use_orphan) o.no_orphan = false;
     {   // record fields print in the order of the MPLP_PRINT_* bits (bam_plcmd.c:185-196,728-795), tags after them in the order given
@@ -1222,11 +1254,12 @@ int main_index(int argc, char **argv)
 
 int main(int argc, char **argv)
 {
-    if (argc < 2) { fprintf(stderr, "Usage: b200samtools <mpileup|depth|coverage|bedcov|gl|counts|index> [options]\n"); return 1; }
+    if (argc < 2) { fprintf(stderr, "Usage: b200samtools <mpileup|depth|coverage|bedcov|gl|counts|indels|index> [options]\n"); return 1; }
     std::string cmd = argv[1];
     if (cmd == "mpileup") return main_mpileup(argc - 1, argv + 1, MP_TEXT);
     if (cmd == "gl") return main_mpileup(argc - 1, argv + 1, MP_GL);
     if (cmd == "counts") return main_mpileup(argc - 1, argv + 1, MP_COUNTS);
+    if (cmd == "indels") return main_mpileup(argc - 1, argv + 1, MP_INDELS);
     if (cmd == "depth") return main_depth(argc - 1, argv + 1);
     if (cmd == "coverage") return main_coverage(argc - 1, argv + 1);
     if (cmd == "bedcov") return main_bedcov(argc - 1, argv + 1);

@@ -364,6 +364,26 @@ PLP_HD int mp_entry_size(const MpConf &cf, const ReadDesc &d, const uint32_t *cg
     return sz;
 }
 
+// the symbols of the insertion after the entry (the ins_scan count of them): the read's IUPAC bases, upper or lower case,
+// 'N' past l_qseq, and `pad` for each P op (bam_plcmd.c:118-145).  The text writes them as the strand shows them; the
+// indel alleles (mpileup_indel.cuh) take the forward-strand form, upper case with '*' pads.
+PLP_HD char *ins_symbols(const View &v, const ReadDesc &d, const uint32_t *cg, const Ent &e, bool lower, char pad, char *p)
+{
+    int j = 1;
+    for (int kk = e.k + 1; kk < (int)d.n_cigar; ++kk) {
+        int op = cg[kk] & 0xf, l = (int)(cg[kk] >> 4);
+        if (op == OP_P) { for (int i = 0; i < l; ++i) *p++ = pad; }
+        else if (op == OP_I) {
+            for (int i = 0; i < l; ++i, ++j) {
+                int q = e.qpos + j - (int)e.is_del;
+                char b = q < d.l_qseq ? "=ACMGRSVTWYHKDBN"[base4(v.seq4, d.qoff, q)] : 'N';
+                *p++ = lower ? lo(b) : up(b);
+            }
+        } else break;
+    }
+    return p;
+}
+
 PLP_HD int mp_entry_write(const View &v, const MpConf &cf, const ReadDesc &d, const uint32_t *cg, const Ent &e,
                           int32_t c, char *p)
 {
@@ -376,20 +396,7 @@ PLP_HD int mp_entry_write(const View &v, const MpConf &cf, const ReadDesc &d, co
     if (e.indel > 0) {
         int len = ins_scan(d, cg, e.k, del_len);
         if (cf.no_ins < 2) { *p++ = '+'; p += put_u64(p, (uint64_t)len); }
-        if (!cf.no_ins) {
-            int j = 1;
-            for (int kk = e.k + 1; kk < (int)d.n_cigar; ++kk) {
-                int op = cg[kk] & 0xf, l = (int)(cg[kk] >> 4);
-                if (op == OP_P) { for (int i = 0; i < l; ++i) *p++ = (rev && cf.rev_del) ? '#' : '*'; }
-                else if (op == OP_I) {
-                    for (int i = 0; i < l; ++i, ++j) {
-                        int q = e.qpos + j - (int)e.is_del;
-                        char b = q < d.l_qseq ? "=ACMGRSVTWYHKDBN"[base4(v.seq4, d.qoff, q)] : 'N';
-                        *p++ = rev ? lo(b) : up(b);
-                    }
-                } else break;
-            }
-        }
+        if (!cf.no_ins) p = ins_symbols(v, d, cg, e, rev, (rev && cf.rev_del) ? '#' : '*', p);
     }
     if (del_len > 0) {
         if (cf.no_del < 2) { *p++ = '-'; p += put_u64(p, (uint64_t)del_len); }
@@ -413,6 +420,14 @@ PLP_HD int ref_chan(char ch)
 {
     switch (up(ch)) { case 'A': return CNT_A; case 'C': return CNT_C; case 'G': return CNT_G; case 'T': return CNT_T; default: return CNT_N; }
 }
+// the indel tokens mp_entry_write prints after the entry of read d (cursor e): returns the symbol count of its "+n" (-1:
+// none; a "+0" is possible on odd CIGARs such as 5M0P1S1I), *del_len the length of its "-n" (0: none).  The caller applies
+// -Q first.
+PLP_HD int mp_entry_indel(const ReadDesc &d, const uint32_t *cg, const Ent &e, int &del_len)
+{
+    del_len = e.indel < 0 ? -e.indel : 0;
+    return e.indel > 0 ? ins_scan(d, cg, e.k, del_len) : -1;
+}
 // the entry of read d at column c (cursor e), as counts: bits 0-3 its kind (CNT_A .. CNT_SKIP), bit 4 a "+n" follows, bit 5
 // a "-n" follows -- what mp_entry_write prints for it.  The caller applies -Q first: a failing entry prints nothing.
 enum { CNT_BIT_INS = 16, CNT_BIT_DEL = 32 };
@@ -421,10 +436,35 @@ PLP_HD int mp_entry_channel(const View &v, const ReadDesc &d, const uint32_t *cg
     int x;
     if (e.is_del) x = e.is_refskip ? CNT_SKIP : CNT_DEL;
     else { const int ch = mp_entry_base(v, d, e, c); x = ch ? nt16_int_of(ch) : ref_chan(ref_char(v, c)); }
-    int del_len = -e.indel;
-    if (e.indel > 0) { ins_scan(d, cg, e.k, del_len); x |= CNT_BIT_INS; }
+    int del_len;
+    if (mp_entry_indel(d, cg, e, del_len) >= 0) x |= CNT_BIT_INS;
     if (del_len > 0) x |= CNT_BIT_DEL;
     return x;
+}
+
+// ---- indel alleles of the entries (mpileup_indel.cuh): the distinct "+n..." / "-n" tokens of one (column, file) ---------
+// An allele is its signed length (>= 0: an insertion of that many symbols, forward-strand form from ins_symbols; < 0: a
+// deletion of -len reference bases, which name it by length alone) and, for an insertion, the symbol bytes.  Two tokens are
+// one allele exactly when indel_allele_equal says so; indel_key only filters and spreads candidates (it may collide).
+PLP_HD bool indel_allele_equal(int32_t len_a, const char *sym_a, int32_t len_b, const char *sym_b)
+{
+    if (len_a != len_b) return false;
+    for (int32_t i = 0; i < len_a; ++i) if (sym_a[i] != sym_b[i]) return false;
+    return true;
+}
+// Insertions of up to 12 symbols pack exactly (length in bits 60-63, five bits per symbol: the nt16 code, '*' = 16); longer
+// ones and deletions hash (FNV-1a over the length and the bytes).  key_mask narrows the key so that tests can force collisions.
+PLP_HD uint64_t indel_key(int32_t len, const char *sym, uint64_t key_mask)
+{
+    uint64_t k;
+    if (len >= 0 && len <= 12) {
+        k = (uint64_t)len << 60;
+        for (int32_t i = 0; i < len; ++i) k |= (uint64_t)(sym[i] == '*' ? 16 : nt16_of((unsigned char)sym[i])) << (5 * i);
+    } else {
+        k = 0xcbf29ce484222325ull ^ (uint64_t)(uint32_t)len;
+        for (int32_t i = 0; i < len; ++i) k = (k ^ (uint8_t)sym[i]) * 0x100000001b3ull;
+    }
+    return k & key_mask;
 }
 
 // per (column, file) sizes

@@ -21,8 +21,11 @@ EXPORTS = ['b200_engine_create', 'b200_engine_destroy', 'b200_last_error', 'b200
            'b200_fetch_mapq_keep', 'b200_pileup_entries', 'b200_last_kernel_ms', 'b200_last_stage_ms', 'b200_set_keep_raw', 'b200_restage', 'b200_last_stage_device_ms',
            'b200_launch_count', 'b200_last_mpileup_parts_ms', 'b200_gl_rng_draws', 'b200_last_baq_ms',
            'b200_errmod_cal', 'b200_glfgen', 'b200_cap_mapq', 'b200_mpileup_text_bound', 'b200_depth_text_bound', 'b200_bedcov',
-           'b200_mpileup_counts']
+           'b200_mpileup_counts', 'b200_mpileup_indels', 'b200_fetch_indels']
 COUNT_PLANES = 19   # b200_mpileup_counts: per file A C G T N del skip +ins -del, forward then reverse strand, then n_plp
+# b200_indel_t, one row of b200_mpileup_indels: len >= 0 an insertion of len symbols at seq[seq_off:], < 0 a deletion of -len
+INDEL_DTYPE = np.dtype([('col', '<i4'), ('file', '<i4'), ('len', '<i4'), ('fwd', '<u4'), ('rev', '<u4'), ('pad', '<u4'),
+                        ('seq_off', '<u8')])
 
 
 class Batch(C.Structure):
@@ -92,6 +95,8 @@ def load_library():
         lib.b200_coverage.argtypes = [C.c_void_p, C.POINTER(CoverageConf), C.POINTER(CoverageSums)]
         lib.b200_glf.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_mpileup_counts.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64)]
+        lib.b200_mpileup_indels.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_uint64)]
+        lib.b200_fetch_indels.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
         lib.b200_fetch_qual.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_fetch_mapq_keep.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_pileup_entries.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -257,6 +262,29 @@ class Engine:
         if self.lib.b200_mpileup_counts(self.h, min_baseQ, C.c_void_p(out.data_ptr()), shape[2], C.byref(n)) != 0:
             self._err('b200_mpileup_counts')
         return out
+
+    def mpileup_indels(self, min_baseQ=13, device=False):
+        """Per-column indel alleles of the staged window (b200_mpileup_indels): (rows, symbols).  By default a numpy structured
+        array of INDEL_DTYPE and the insertion symbols as uint8 bytes; with device=True an int32 [n, 8] CUDA tensor (the
+        same 32-byte rows) and a uint8 CUDA tensor on the handle's device, filled on the device."""
+        n, nb = C.c_int64(0), C.c_uint64(0)
+        if self.lib.b200_mpileup_indels(self.h, min_baseQ, C.byref(n), C.byref(nb)) != 0:
+            self._err('b200_mpileup_indels')
+        if not device:
+            rows, seq = np.zeros(n.value, INDEL_DTYPE), np.zeros(nb.value, np.uint8)
+            if self.lib.b200_fetch_indels(self.h, _ptr(rows) if n.value else None, n.value,
+                                          _ptr(seq) if nb.value else None, nb.value) != 0:
+                self._err('b200_fetch_indels')
+            return rows, seq
+        import torch
+        dev = torch.device('cuda', self.device)
+        rows = torch.empty((n.value, INDEL_DTYPE.itemsize // 4), dtype=torch.int32, device=dev)
+        seq = torch.empty(nb.value, dtype=torch.uint8, device=dev)
+        torch.cuda.current_stream(dev).synchronize()   # the engine writes on its own stream
+        if self.lib.b200_fetch_indels(self.h, C.c_void_p(rows.data_ptr()) if n.value else None, n.value,
+                                      C.c_void_p(seq.data_ptr()) if nb.value else None, nb.value) != 0:
+            self._err('b200_fetch_indels')
+        return rows, seq
 
     def fetch_qual(self, nbytes):
         q = np.zeros(nbytes, np.uint8)
