@@ -26,6 +26,8 @@
  *   b200_glf()            bcf_call_glfgen + errmod_cal    bam2bcf.c:65-123 (+ htslib errmod.c)
  *   b200_mpileup_counts() pileup_seq, as numbers           bam_plcmd.c:54-169 -> per-column strand-split base / indel counts
  *   b200_mpileup_indels() pileup_seq's +n / -n tokens      bam_plcmd.c:54-169 -> per-column indel alleles, strand-split support
+ *   b200_mpileup_qsums()  the qual and -s columns          bam_plcmd.c:674-688, :728-748 -> per-column BQ / MQ sums, MQ0
+ *   b200_indel_qsums()    (the same, per indel allele)     -> BQ / MQ sums and MQ0 counts of each allele's entries
  *   b200_pileup_entries() bam_plp64_next/resolve_cigar2   (htslib sam.c) -> arrays of bam_pileup1_t fields
  *
  * Conventions: plain C, caller-owned host buffers, int return codes (0 ok,
@@ -254,6 +256,27 @@ typedef struct {
 } b200_indel_t;
 int b200_mpileup_indels(b200_engine_t *e, int32_t min_baseQ, int64_t *n_alleles, uint64_t *n_seq_bytes);
 int b200_fetch_indels(b200_engine_t *e, b200_indel_t *alleles, size_t cap_alleles, char *seq, size_t cap_seq);
+/* per-column quality sums of the mpileup column stage, beside the counts: what a parser of the `mpileup --reverse-del -s`
+ * text adds up over the entries that pass -Q (min_baseQ).  An entry's BQ is its quality character minus 33 (the quality
+ * after BAQ, -6 and the overlap tweak, clamped at 93 as the text prints '~'), its MQ its -s character minus 33 (the mapq
+ * after -C, clamped at 93), its MQ0 1 where that character is '!' (mapq 0).  Per file 42 uint32 planes, laid out, sized and
+ * delivered exactly as those of b200_mpileup_counts: out[(f * 42 + k) * n + c], zero where a column is empty; out == NULL
+ * computes only; host or device memory; cap_cols < n returns -2; needs a batch staged in B200_MODE_MPILEUP.  Plane
+ *   k = s * 14 + r * 7 + kind,   s: 0 BQ sum, 1 MQ sum, 2 MQ0 count;  r: 0 forward, 1 reverse strand;
+ *                                kind: 0-6 A C G T N deletion skip, as planes r * 9 + kind of b200_mpileup_counts
+ * Sums are exact while a column has at most 46182444 reads (93 times that fits in 32 bits); the call fails on a deeper one
+ * (possible only without a max-depth limit) instead of wrapping.  b200_last_kernel_ms() covers it. */
+#define B200_QSUM_PLANES 42
+int b200_mpileup_qsums(b200_engine_t *e, int32_t min_baseQ, uint32_t *out, size_t cap_cols, int64_t *n_cols);
+/* quality sums beside the indel table: row j holds, per strand, the BQ and MQ sums and the MQ0 count (as above) of the
+ * entries that carry allele j of the last b200_mpileup_indels since the batch was staged (with that call's -Q), so fwd and
+ * rev of row j are the counts they are taken over.  Refused without such a table, as b200_fetch_indels is.  out == NULL
+ * computes only; otherwise host or device memory (a device buffer must be on the handle's device); cap_rows below the row
+ * count returns -2.  b200_last_kernel_ms() covers it.  24 bytes per row (a uint32 [n, 6] view). */
+typedef struct {
+    uint32_t bq_fwd, bq_rev, mq_fwd, mq_rev, mq0_fwd, mq0_rev;
+} b200_indel_qsum_t;
+int b200_indel_qsums(b200_engine_t *e, b200_indel_qsum_t *out, size_t cap_rows);
 /* htslib's per-column / per-read entry points on the device (tier T1 support; one column or one small batch per call):
  *   b200_errmod_cal   errmod_cal(em, n, m, bases, q) of htslib errmod.c (callers bam2bcf.c:121, phase.c:754, cut_target.c:84):
  *                     `bases` (q<<5|strand<<4|allele) is left sorted like the reference leaves it, q[m*m] receives the

@@ -905,15 +905,20 @@ extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c,
     return text_end(e, e->col_off + nt, bound, out, out_cap, out_len);
 }
 
-extern "C" int b200_mpileup_counts(b200_engine_t *e, int32_t min_baseQ, uint32_t *out, size_t cap_cols, int64_t *n_cols)
+// The planes of b200_mpileup_counts and b200_mpileup_qsums: checks, destination, the kernel (launch(blocks, view, n_groups,
+// dst): k_mp_counts or k_mp_qsums), the copy to host memory.  deep: the d_misc slot where k_mp_qsums flags a column too
+// deep for its sums, or nullptr.
+template <class Launch>
+static int col_planes(b200_engine *e, const char *what, const char *buf, int planes, uint32_t *out, size_t cap_cols, int64_t *n_cols,
+                      unsigned long long *deep, Launch launch)
 {
     if (!e || !e->staged) { if (e) snprintf(e->err, sizeof e->err, "no staged batch"); return -1; }
-    if (e->sconf.mode != B200_MODE_MPILEUP) { snprintf(e->err, sizeof e->err, "mpileup counts need a batch staged in B200_MODE_MPILEUP"); return -1; }
+    if (e->sconf.mode != B200_MODE_MPILEUP) { snprintf(e->err, sizeof e->err, "mpileup %s need a batch staged in B200_MODE_MPILEUP", what); return -1; }
     CK(cudaSetDevice(e->device));
     View v; fill_view(e, v, nullptr, nullptr, 0, 0, 1);
     const int64_t n = v.ncols;
     *n_cols = n; e->last_kernel_ms = 0;
-    if (out && cap_cols < (size_t)n) { snprintf(e->err, sizeof e->err, "count buffer too small: need %lld columns", (long long)n); return -2; }
+    if (out && cap_cols < (size_t)n) { snprintf(e->err, sizeof e->err, "%s buffer too small: need %lld columns", buf, (long long)n); return -2; }
     if (n == 0) return 0;
     // the kernel writes straight into a caller's device buffer; host memory gets the planes through the handle's buffer
     uint32_t *dst = nullptr;
@@ -921,21 +926,40 @@ extern "C" int b200_mpileup_counts(b200_engine_t *e, int32_t min_baseQ, uint32_t
         cudaPointerAttributes a;
         CK(cudaPointerGetAttributes(&a, out));
         if (a.type == cudaMemoryTypeDevice) {
-            if (a.device != e->device) { snprintf(e->err, sizeof e->err, "count buffer is on device %d, the handle on device %d", a.device, e->device); return -1; }
+            if (a.device != e->device) { snprintf(e->err, sizeof e->err, "%s buffer is on device %d, the handle on device %d", buf, a.device, e->device); return -1; }
             dst = out;
         } else if (a.type == cudaMemoryTypeManaged) dst = out;
     }
-    const size_t words = (size_t)e->n_files * CNT_PLANES * (size_t)n;
+    const size_t words = (size_t)e->n_files * (size_t)planes * (size_t)n;
     if (!dst) { ENSURE(cnt, words); dst = e->cnt; }
     const int64_t warps = (int64_t)e->n_files * ((n + 31) / 32);
+    if (deep) CK(cudaMemsetAsync(deep, 0, 8, e->stream));
     CK(cudaEventRecord(e->ev0, e->stream));
-    k_mp_counts<<<nblk(warps, CNT_WARPS), CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, (int32_t)((n + 31) / 32), dst); e->launches++;
+    launch(nblk(warps, CNT_WARPS), v, (int32_t)((n + 31) / 32), dst); e->launches++;
     CK(cudaEventRecord(e->ev1, e->stream));
     if (out && dst != out) CK(cudaMemcpyAsync(out, dst, words * 4, cudaMemcpyDeviceToHost, e->stream));
+    unsigned long long h_deep = 0;
+    if (deep) CK(cudaMemcpyAsync(&h_deep, deep, 8, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     CK(cudaGetLastError());
+    if (h_deep) { snprintf(e->err, sizeof e->err, "a column has more than %u reads: its %s would not fit in 32 bits", QS_MAX_DEPTH, what); return -1; }
     float ms = 0; cudaEventElapsedTime(&ms, e->ev0, e->ev1); e->last_kernel_ms = ms;
     return 0;
+}
+
+extern "C" int b200_mpileup_counts(b200_engine_t *e, int32_t min_baseQ, uint32_t *out, size_t cap_cols, int64_t *n_cols)
+{
+    return col_planes(e, "counts", "count", CNT_PLANES, out, cap_cols, n_cols, nullptr, [&](int blocks, const View &v, int32_t n_groups, uint32_t *dst) {
+        k_mp_counts<<<blocks, CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, dst);
+    });
+}
+
+extern "C" int b200_mpileup_qsums(b200_engine_t *e, int32_t min_baseQ, uint32_t *out, size_t cap_cols, int64_t *n_cols)
+{
+    unsigned long long *deep = e ? e->d_misc + MISC_QSUM_DEEP : nullptr;
+    return col_planes(e, "quality sums", "quality sum", QS_PLANES, out, cap_cols, n_cols, deep, [&](int blocks, const View &v, int32_t n_groups, uint32_t *dst) {
+        k_mp_qsums<<<blocks, CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, dst, deep);
+    });
 }
 
 // Test knob: B200_INDEL_KEY_BITS=k keeps the low k bits of every allele key, so different insertions share keys and the
@@ -952,7 +976,7 @@ extern "C" int b200_mpileup_indels(b200_engine_t *e, int32_t min_baseQ, int64_t 
     if (!e || !e->staged) { if (e) snprintf(e->err, sizeof e->err, "no staged batch"); return -1; }
     if (e->sconf.mode != B200_MODE_MPILEUP) { snprintf(e->err, sizeof e->err, "mpileup indels need a batch staged in B200_MODE_MPILEUP"); return -1; }
     CK(cudaSetDevice(e->device));
-    e->ind_ready = false; e->ind_n = 0; e->ind_nseq = 0; e->last_kernel_ms = 0;
+    e->ind_ready = false; e->ind_n = 0; e->ind_nseq = 0; e->ind_nev = 0; e->last_kernel_ms = 0;
     *n_alleles = 0; *n_seq_bytes = 0;
     View v; fill_view(e, v, nullptr, nullptr, 0, 0, 1);
     const int64_t n = v.ncols, segs = n * e->n_files;
@@ -1001,7 +1025,7 @@ extern "C" int b200_mpileup_indels(b200_engine_t *e, int32_t min_baseQ, int64_t 
         return -1;
     }
     float ms = 0; cudaEventElapsedTime(&ms, e->ev0, e->ev1); e->last_kernel_ms = ms;
-    e->ind_n = h_n; e->ind_nseq = h_seq; e->ind_ready = true;
+    e->ind_n = h_n; e->ind_nseq = h_seq; e->ind_nev = h_ev; e->ind_ready = true;
     *n_alleles = h_n; *n_seq_bytes = h_seq;
     return 0;
 }
@@ -1036,6 +1060,37 @@ extern "C" int b200_fetch_indels(b200_engine_t *e, b200_indel_t *alleles, size_t
         CK(cudaMemcpyAsync(seq, e->ind_seq, e->ind_nseq, cudaMemcpyDefault, e->stream));
     }
     CK(cudaStreamSynchronize(e->stream));
+    return 0;
+}
+
+extern "C" int b200_indel_qsums(b200_engine_t *e, b200_indel_qsum_t *out, size_t cap_rows)
+{
+    if (!e || !e->staged || !e->ind_ready) {
+        if (e) snprintf(e->err, sizeof e->err, "no indel table: call b200_mpileup_indels on the staged batch first");
+        return -1;
+    }
+    CK(cudaSetDevice(e->device));
+    e->last_kernel_ms = 0;
+    if (out && cap_rows < (size_t)e->ind_n) { snprintf(e->err, sizeof e->err, "quality sum buffer too small: need %lld rows", (long long)e->ind_n); return -2; }
+    if (out && e->ind_n && check_dst(e, out, "quality sum")) return -1;
+    if (e->ind_n == 0) return 0;
+    // the events, hash slots, allele indices and rows of the table are still those b200_mpileup_indels left in HBM
+    ENSURE(ind_qs, (size_t)e->ind_n);
+    View v; fill_view(e, v, nullptr, nullptr, 0, 0, 1);
+    unsigned long long *deep = e->d_misc + MISC_QSUM_DEEP;
+    CK(cudaEventRecord(e->ev0, e->stream));
+    CK(cudaMemsetAsync(e->ind_qs, 0, (size_t)e->ind_n * sizeof(b200_indel_qsum_t), e->stream));
+    CK(cudaMemsetAsync(deep, 0, 8, e->stream));
+    k_ind_qsums<<<nblk(e->ind_nev, 256), 256, 0, e->stream>>>(v, (const IndelEv *)e->ind_ev, e->ind_nev, e->ind_tbl, e->ind_slot, e->ind_aidx,
+                                                            e->ind_tab, e->ind_qs, deep); e->launches++;
+    CK(cudaEventRecord(e->ev1, e->stream));
+    if (out) CK(cudaMemcpyAsync(out, e->ind_qs, (size_t)e->ind_n * sizeof(b200_indel_qsum_t), cudaMemcpyDefault, e->stream));
+    unsigned long long h_deep = 0;
+    CK(cudaMemcpyAsync(&h_deep, deep, 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    CK(cudaGetLastError());
+    if (h_deep) { snprintf(e->err, sizeof e->err, "an indel allele has more than %u entries on one strand: its quality sums would not fit in 32 bits", QS_MAX_DEPTH); return -1; }
+    float ms = 0; cudaEventElapsedTime(&ms, e->ev0, e->ev1); e->last_kernel_ms = ms;
     return 0;
 }
 

@@ -1,26 +1,29 @@
-// mpileup_cnt.cuh -- per-column base and indel counts of the mpileup column stage (b200_mpileup_counts).
-// Included by engine.cu.
+// mpileup_cnt.cuh -- per-column planes of the mpileup column stage: base and indel counts (b200_mpileup_counts) and quality
+// sums (b200_mpileup_qsums).  Included by engine.cu.
 //
-// What a parser of the "--reverse-del" text would count, kept as numbers in HBM: per file CNT_PLANES planes of uint32
-// (plp_core.h mp_entry_channel), out[f][plane][c] over the columns [0, ncols) of the window.
+// What a parser of the "--reverse-del" text would count, or add up from its "-s" text, kept as numbers in HBM: per file
+// CNT_PLANES (plp_core.h mp_entry_channel) or QS_PLANES (mp_entry_qs) planes of uint32, out[f][plane][c] over the columns
+// [0, ncols) of the window.
 //
 // One warp per (file, 32-column group), lane = column: the warp walks the group's reads (read_range, far-reaching reads
 // included) and every lane loads the same descriptor (a broadcast).  A simple read resolves by arithmetic, so the lanes'
 // quality and base loads are consecutive bytes / nibbles of one read; other reads go through the CIGAR cursor.  The
 // counters live in shared memory, [plane][lane] per warp: each lane owns one column of every plane (no atomics, no bank
 // conflicts), and a plane index never selects a register (local memory, DESIGN section 7).  The planes leave as coalesced
-// 128-byte rows.
+// 128-byte rows.  Both kernels run the one walk mp_col_planes; they differ in what an entry that passes -Q adds (`add`)
+// and in what the lane does with the column's n_plp (`fin`).
 constexpr int CNT_WARPS = 4;
 
-__global__ void __launch_bounds__(CNT_WARPS * 32) k_mp_counts(View v, int32_t min_baseQ, int32_t n_groups, uint32_t *out)
+template <int P, class Add, class Fin>
+__device__ __forceinline__ void mp_col_planes(const View &v, int32_t min_baseQ, int32_t n_groups, uint32_t *out,
+                                              uint32_t (*s_all)[P][32], Add add, Fin fin)
 {
-    __shared__ uint32_t s_cnt[CNT_WARPS][CNT_PLANES][32];
     const int lane = threadIdx.x & 31, wl = threadIdx.x >> 5;
     const int64_t w = (int64_t)blockIdx.x * CNT_WARPS + wl;
     if (w >= (int64_t)n_groups * v.n_files) return;        // whole warps: nothing below synchronises across warps
     const int f = (int)(w / n_groups), g = (int)(w % n_groups);
-    uint32_t (*s)[32] = s_cnt[wl];
-    for (int k = 0; k < CNT_PLANES; ++k) s[k][lane] = 0;
+    uint32_t (*s)[32] = s_all[wl];
+    for (int k = 0; k < P; ++k) s[k][lane] = 0;
     const int32_t c = g * 32 + lane;
     const ReadRange rr = read_range(v, f, g);
     uint32_t nplp = 0;
@@ -31,16 +34,43 @@ __global__ void __launch_bounds__(CNT_WARPS * 32) k_mp_counts(View v, int32_t mi
         ++nplp;
         Ent e;
         resolve(v, d, c, e);
-        if (ent_qual(v, d, e) < min_baseQ) continue;
-        const int x = mp_entry_channel(v, d, v.cigar + d.cig_off, e, c);
-        const int o = (d.fl & RD_REV) ? CNT_REV : 0;
-        ++s[o + (x & 15)][lane];
-        if (x & CNT_BIT_INS) ++s[o + CNT_INS_NEXT][lane];
-        if (x & CNT_BIT_DEL) ++s[o + CNT_DEL_NEXT][lane];
+        const int q = ent_qual(v, d, e);
+        if (q < min_baseQ) continue;
+        add(s, lane, d, e, c, q);
     }
-    s[CNT_NPLP][lane] = nplp;
+    fin(s, lane, nplp);
     if (c >= v.ncols) return;
-    uint32_t *p = out + (int64_t)f * CNT_PLANES * v.ncols + c;
+    uint32_t *p = out + (int64_t)f * P * v.ncols + c;
 #pragma unroll
-    for (int k = 0; k < CNT_PLANES; ++k) p[(int64_t)k * v.ncols] = s[k][lane];
+    for (int k = 0; k < P; ++k) p[(int64_t)k * v.ncols] = s[k][lane];
+}
+
+__global__ void __launch_bounds__(CNT_WARPS * 32) k_mp_counts(View v, int32_t min_baseQ, int32_t n_groups, uint32_t *out)
+{
+    __shared__ uint32_t s_cnt[CNT_WARPS][CNT_PLANES][32];
+    mp_col_planes<CNT_PLANES>(v, min_baseQ, n_groups, out, s_cnt,
+        [&](uint32_t (*s)[32], int lane, const ReadDesc &d, const Ent &e, int32_t c, int) {
+            const int x = mp_entry_channel(v, d, v.cigar + d.cig_off, e, c);
+            const int o = (d.fl & RD_REV) ? CNT_REV : 0;
+            ++s[o + (x & 15)][lane];
+            if (x & CNT_BIT_INS) ++s[o + CNT_INS_NEXT][lane];
+            if (x & CNT_BIT_DEL) ++s[o + CNT_DEL_NEXT][lane];
+        },
+        [&](uint32_t (*s)[32], int lane, uint32_t nplp) { s[CNT_NPLP][lane] = nplp; });
+}
+
+// deep: set where a column has more than QS_MAX_DEPTH reads (a sum could wrap); the call then fails
+__global__ void __launch_bounds__(CNT_WARPS * 32) k_mp_qsums(View v, int32_t min_baseQ, int32_t n_groups, uint32_t *out,
+                                                             unsigned long long *deep)
+{
+    __shared__ uint32_t s_qs[CNT_WARPS][QS_PLANES][32];
+    mp_col_planes<QS_PLANES>(v, min_baseQ, n_groups, out, s_qs,
+        [&](uint32_t (*s)[32], int lane, const ReadDesc &d, const Ent &e, int32_t c, int q) {
+            const EntQs x = mp_entry_qs(q, d);
+            const int k = ((d.fl & RD_REV) ? QS_REV : 0) + (mp_entry_channel(v, d, v.cigar + d.cig_off, e, c) & 15);
+            s[k][lane] += x.bq;
+            s[QS_MQ + k][lane] += x.mq;
+            s[QS_MQ0 + k][lane] += x.mq0;
+        },
+        [&](uint32_t (*)[32], int, uint32_t nplp) { if (nplp > QS_MAX_DEPTH) *deep = 1ull; });
 }

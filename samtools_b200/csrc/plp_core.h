@@ -442,6 +442,24 @@ PLP_HD int mp_entry_channel(const View &v, const ReadDesc &d, const uint32_t *cg
     return x;
 }
 
+// ---- per-column quality sums of the entries (mpileup_cnt.cuh, mpileup_indel.cuh): what a parser of the "-s" text adds ------
+// Planes per file: the BQ sums of kinds 0-6 (mp_entry_channel & 15) of forward-strand entries, the same for reverse-strand
+// ones (+ QS_REV), then the MQ sums (+ QS_MQ) and the MQ0 counts (+ QS_MQ0) in the same order.
+enum { QS_REV = 7, QS_MQ = 14, QS_MQ0 = 28, QS_PLANES = B200_QSUM_PLANES };
+constexpr uint32_t QS_MAX_DEPTH = 46182444;   // floor((2^32 - 1) / 93): a sum over this many entries stays exact in 32 bits
+struct EntQs { uint32_t bq, mq, mq0; };
+// an entry that passes -Q, as the text prints it: q (ent_qual) is its quality character minus 33, clamped at 93 like the '~'
+// an overlap-summed quality prints as; the descriptor's mapq (after -C) its "-s" character minus 33, also clamped at 93; MQ0
+// is that character being '!'
+PLP_HD EntQs mp_entry_qs(int q, const ReadDesc &d)
+{
+    EntQs r;
+    r.bq = (uint32_t)(q < 93 ? q : 93);
+    r.mq = d.mapq < 93 ? d.mapq : 93u;
+    r.mq0 = d.mapq == 0;
+    return r;
+}
+
 // ---- indel alleles of the entries (mpileup_indel.cuh): the distinct "+n..." / "-n" tokens of one (column, file) ---------
 // An allele is its signed length (>= 0: an insertion of that many symbols, forward-strand form from ins_symbols; < 0: a
 // deletion of -len reference bases, which name it by length alone) and, for an insertion, the symbol bytes.  Two tokens are

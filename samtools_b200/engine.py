@@ -21,8 +21,11 @@ EXPORTS = ['b200_engine_create', 'b200_engine_destroy', 'b200_last_error', 'b200
            'b200_fetch_mapq_keep', 'b200_pileup_entries', 'b200_last_kernel_ms', 'b200_last_stage_ms', 'b200_set_keep_raw', 'b200_restage', 'b200_last_stage_device_ms',
            'b200_launch_count', 'b200_last_mpileup_parts_ms', 'b200_gl_rng_draws', 'b200_last_baq_ms',
            'b200_errmod_cal', 'b200_glfgen', 'b200_cap_mapq', 'b200_mpileup_text_bound', 'b200_depth_text_bound', 'b200_bedcov',
-           'b200_mpileup_counts', 'b200_mpileup_indels', 'b200_fetch_indels']
+           'b200_mpileup_counts', 'b200_mpileup_indels', 'b200_fetch_indels', 'b200_mpileup_qsums', 'b200_indel_qsums']
 COUNT_PLANES = 19   # b200_mpileup_counts: per file A C G T N del skip +ins -del, forward then reverse strand, then n_plp
+QSUM_PLANES = 42    # b200_mpileup_qsums: per file BQ sums, MQ sums, MQ0 counts, each of A C G T N del skip, forward then reverse
+# b200_indel_qsum_t, one row of b200_indel_qsums beside the row of b200_mpileup_indels
+INDEL_QSUM_FIELDS = ('bq_fwd', 'bq_rev', 'mq_fwd', 'mq_rev', 'mq0_fwd', 'mq0_rev')
 # b200_indel_t, one row of b200_mpileup_indels: len >= 0 an insertion of len symbols at seq[seq_off:], < 0 a deletion of -len
 INDEL_DTYPE = np.dtype([('col', '<i4'), ('file', '<i4'), ('len', '<i4'), ('fwd', '<u4'), ('rev', '<u4'), ('pad', '<u4'),
                         ('seq_off', '<u8')])
@@ -97,6 +100,8 @@ def load_library():
         lib.b200_mpileup_counts.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64)]
         lib.b200_mpileup_indels.argtypes = [C.c_void_p, C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_uint64)]
         lib.b200_fetch_indels.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+        lib.b200_mpileup_qsums.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64)]
+        lib.b200_indel_qsums.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_fetch_qual.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_fetch_mapq_keep.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_pileup_entries.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -147,6 +152,7 @@ class Engine:
         self.device = device
         self._keep = None
         self._n_files = self._n_cols = 0
+        self._n_alleles = 0   # rows of the last mpileup_indels on the staged batch
 
     def close(self):
         if self.h:
@@ -181,6 +187,7 @@ class Engine:
         st = StageStats()
         self._keep = (soa, name)
         self._n_files = b.n_files
+        self._n_alleles = 0
         if self.lib.b200_stage(self.h, C.byref(b), C.byref(conf), C.byref(st)) != 0:
             self._err('b200_stage')
         self._n_cols = st.n_cols
@@ -193,6 +200,7 @@ class Engine:
 
     def restage(self):
         st = StageStats()
+        self._n_alleles = 0
         if self.lib.b200_restage(self.h, C.byref(st)) != 0:
             self._err('b200_restage')
         self._n_cols = st.n_cols
@@ -242,16 +250,13 @@ class Engine:
         k = n.value
         return pos[:k], nb[:k * n_files].reshape(k, n_files), qs[:k * n_files * 4].reshape(k, n_files, 4), p25[:k * n_files * 25].reshape(k, n_files, 25)
 
-    def mpileup_counts(self, min_baseQ=13, out=None):
-        """Per-column strand-split base and indel counts of the staged window (b200_mpileup_counts): a numpy uint32
-        [n_files, 19, n] array, or, given `out`, a contiguous torch.int32 CUDA tensor of that shape on the handle's device,
-        filled in place on the device (and returned)."""
+    def _planes(self, fn, planes, min_baseQ, out):
         n = C.c_int64(0)
-        shape = (self._n_files, COUNT_PLANES, self._n_cols)     # the stage's n_cols are the columns of the planes
+        shape = (self._n_files, planes, self._n_cols)     # the stage's n_cols are the columns of the planes
         if out is None:
             a = np.zeros(shape, np.uint32)
-            if self.lib.b200_mpileup_counts(self.h, min_baseQ, _ptr(a), shape[2], C.byref(n)) != 0:
-                self._err('b200_mpileup_counts')
+            if getattr(self.lib, fn)(self.h, min_baseQ, _ptr(a), shape[2], C.byref(n)) != 0:
+                self._err(fn)
             return a
         import torch
         if out.dtype != torch.int32 or not out.is_cuda or not out.is_contiguous() or out.device.index != self.device:
@@ -259,17 +264,31 @@ class Engine:
         if tuple(out.shape) != shape:
             raise ValueError(f'out must have shape {list(shape)}')
         torch.cuda.current_stream(out.device).synchronize()   # the engine writes on its own stream
-        if self.lib.b200_mpileup_counts(self.h, min_baseQ, C.c_void_p(out.data_ptr()), shape[2], C.byref(n)) != 0:
-            self._err('b200_mpileup_counts')
+        if getattr(self.lib, fn)(self.h, min_baseQ, C.c_void_p(out.data_ptr()), shape[2], C.byref(n)) != 0:
+            self._err(fn)
         return out
+
+    def mpileup_counts(self, min_baseQ=13, out=None):
+        """Per-column strand-split base and indel counts of the staged window (b200_mpileup_counts): a numpy uint32
+        [n_files, 19, n] array, or, given `out`, a contiguous torch.int32 CUDA tensor of that shape on the handle's device,
+        filled in place on the device (and returned)."""
+        return self._planes('b200_mpileup_counts', COUNT_PLANES, min_baseQ, out)
+
+    def mpileup_qsums(self, min_baseQ=13, out=None):
+        """Per-column quality sums of the staged window (b200_mpileup_qsums): a numpy uint32 [n_files, 42, n] array of BQ
+        sums, MQ sums and MQ0 counts (plane s * 14 + strand * 7 + kind), or, given `out`, a contiguous torch.int32 CUDA
+        tensor of that shape on the handle's device, filled in place on the device (and returned)."""
+        return self._planes('b200_mpileup_qsums', QSUM_PLANES, min_baseQ, out)
 
     def mpileup_indels(self, min_baseQ=13, device=False):
         """Per-column indel alleles of the staged window (b200_mpileup_indels): (rows, symbols).  By default a numpy structured
         array of INDEL_DTYPE and the insertion symbols as uint8 bytes; with device=True an int32 [n, 8] CUDA tensor (the
         same 32-byte rows) and a uint8 CUDA tensor on the handle's device, filled on the device."""
         n, nb = C.c_int64(0), C.c_uint64(0)
+        self._n_alleles = 0
         if self.lib.b200_mpileup_indels(self.h, min_baseQ, C.byref(n), C.byref(nb)) != 0:
             self._err('b200_mpileup_indels')
+        self._n_alleles = n.value
         if not device:
             rows, seq = np.zeros(n.value, INDEL_DTYPE), np.zeros(nb.value, np.uint8)
             if self.lib.b200_fetch_indels(self.h, _ptr(rows) if n.value else None, n.value,
@@ -285,6 +304,24 @@ class Engine:
                                       C.c_void_p(seq.data_ptr()) if nb.value else None, nb.value) != 0:
             self._err('b200_fetch_indels')
         return rows, seq
+
+    def indel_qsums(self, device=False):
+        """Quality sums of the rows of the last mpileup_indels on the staged batch (b200_indel_qsums), one row per allele in
+        the table's order, columns INDEL_QSUM_FIELDS: a numpy uint32 [n, 6] array, or with device=True an int32 [n, 6] CUDA
+        tensor on the handle's device, filled on the device."""
+        n = self._n_alleles
+        if not device:
+            a = np.zeros((n, len(INDEL_QSUM_FIELDS)), np.uint32)
+            if self.lib.b200_indel_qsums(self.h, _ptr(a) if n else None, n) != 0:
+                self._err('b200_indel_qsums')
+            return a
+        import torch
+        dev = torch.device('cuda', self.device)
+        t = torch.empty((n, len(INDEL_QSUM_FIELDS)), dtype=torch.int32, device=dev)
+        torch.cuda.current_stream(dev).synchronize()   # the engine writes on its own stream
+        if self.lib.b200_indel_qsums(self.h, C.c_void_p(t.data_ptr()) if n else None, n) != 0:
+            self._err('b200_indel_qsums')
+        return t
 
     def fetch_qual(self, nbytes):
         q = np.zeros(nbytes, np.uint8)
