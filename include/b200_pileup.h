@@ -28,6 +28,8 @@
  *   b200_mpileup_indels() pileup_seq's +n / -n tokens      bam_plcmd.c:54-169 -> per-column indel alleles, strand-split support
  *   b200_mpileup_qsums()  the qual and -s columns          bam_plcmd.c:674-688, :728-748 -> per-column BQ / MQ sums, MQ0
  *   b200_indel_qsums()    (the same, per indel allele)     -> BQ / MQ sums and MQ0 counts of each allele's entries
+ *   b200_mpileup_psums()  the --output-BP-5 column         bam_plcmd.c:753-759 -> per-column BP-5 sums and sums of squares
+ *   b200_indel_psums()    (the same, per indel allele)     -> BP-5 sums and sums of squares of each allele's entries
  *   b200_pileup_entries() bam_plp64_next/resolve_cigar2   (htslib sam.c) -> arrays of bam_pileup1_t fields
  *
  * Conventions: plain C, caller-owned host buffers, int return codes (0 ok,
@@ -277,6 +279,28 @@ typedef struct {
     uint32_t bq_fwd, bq_rev, mq_fwd, mq_rev, mq0_fwd, mq0_rev;
 } b200_indel_qsum_t;
 int b200_indel_qsums(b200_engine_t *e, b200_indel_qsum_t *out, size_t cap_rows);
+/* per-column read-position sums of the mpileup column stage, beside the counts: what a parser of the
+ * `mpileup --reverse-del --output-BP-5` text adds up over the entries that pass -Q (min_baseQ).  An entry's BP-5 is the
+ * 5'-based position of its base in the read, the sequencing cycle: qpos + 1 on the forward strand, l_qseq - qpos + is_del
+ * on the reverse strand (signed: <= 0 for a reverse-strand entry of a read without SEQ at -Q 0, as the text prints it).
+ * Per file 28 int64 planes, laid out, sized and delivered exactly as those of b200_mpileup_counts:
+ * out[(f * 28 + k) * n + c], zero where a column is empty; out == NULL computes only; host or device memory;
+ * cap_cols < n returns -2; needs a batch staged in B200_MODE_MPILEUP.  Plane
+ *   k = s * 14 + r * 7 + kind,   s: 0 BP-5 sum, 1 sum of BP-5 squared;  r: 0 forward, 1 reverse strand;
+ *                                kind: 0-6 A C G T N deletion skip, as planes r * 9 + kind of b200_mpileup_counts
+ * so with the count planes they give the mean and the variance of the position.  The BP-5 sums cannot overflow; the call
+ * fails instead of wrapping where a sum of squares would exceed 2^63 - 1.  b200_last_kernel_ms() covers it. */
+#define B200_PSUM_PLANES 28
+int b200_mpileup_psums(b200_engine_t *e, int32_t min_baseQ, int64_t *out, size_t cap_cols, int64_t *n_cols);
+/* read-position sums beside the indel table: row j holds, per strand, the BP-5 sum and the sum of its squares (as above)
+ * of the entries that carry allele j of the last b200_mpileup_indels since the batch was staged (with that call's -Q); an
+ * indel token takes the BP-5 of the entry it follows.  Refusals, destinations and caps as b200_indel_qsums; the call fails
+ * where a sum of squares would exceed 2^63 - 1.  b200_last_kernel_ms() covers it.  32 bytes per row (an int64 [n, 4]
+ * view). */
+typedef struct {
+    int64_t bp5_fwd, bp5_rev, bp5sq_fwd, bp5sq_rev;
+} b200_indel_psum_t;
+int b200_indel_psums(b200_engine_t *e, b200_indel_psum_t *out, size_t cap_rows);
 /* htslib's per-column / per-read entry points on the device (tier T1 support; one column or one small batch per call):
  *   b200_errmod_cal   errmod_cal(em, n, m, bases, q) of htslib errmod.c (callers bam2bcf.c:121, phase.c:754, cut_target.c:84):
  *                     `bases` (q<<5|strand<<4|allele) is left sorted like the reference leaves it, q[m*m] receives the

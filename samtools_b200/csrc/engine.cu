@@ -905,12 +905,12 @@ extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c,
     return text_end(e, e->col_off + nt, bound, out, out_cap, out_len);
 }
 
-// The planes of b200_mpileup_counts and b200_mpileup_qsums: checks, destination, the kernel (launch(blocks, view, n_groups,
-// dst): k_mp_counts or k_mp_qsums), the copy to host memory.  deep: the d_misc slot where k_mp_qsums flags a column too
-// deep for its sums, or nullptr.
-template <class Launch>
-static int col_planes(b200_engine *e, const char *what, const char *buf, int planes, uint32_t *out, size_t cap_cols, int64_t *n_cols,
-                      unsigned long long *deep, Launch launch)
+// The planes of b200_mpileup_counts, b200_mpileup_qsums and b200_mpileup_psums: checks, destination, the kernel
+// (launch(blocks, view, n_groups, dst): k_mp_counts, k_mp_qsums or k_mp_psums), the copy to host memory.  T: the cell type.
+// flag: the d_misc slot where the kernel flags a sum it could not keep exact, or nullptr; the call then fails with flag_msg.
+template <class T, class Launch>
+static int col_planes(b200_engine *e, const char *what, const char *buf, int planes, T *out, size_t cap_cols, int64_t *n_cols,
+                      unsigned long long *flag, const char *flag_msg, Launch launch)
 {
     if (!e || !e->staged) { if (e) snprintf(e->err, sizeof e->err, "no staged batch"); return -1; }
     if (e->sconf.mode != B200_MODE_MPILEUP) { snprintf(e->err, sizeof e->err, "mpileup %s need a batch staged in B200_MODE_MPILEUP", what); return -1; }
@@ -921,7 +921,7 @@ static int col_planes(b200_engine *e, const char *what, const char *buf, int pla
     if (out && cap_cols < (size_t)n) { snprintf(e->err, sizeof e->err, "%s buffer too small: need %lld columns", buf, (long long)n); return -2; }
     if (n == 0) return 0;
     // the kernel writes straight into a caller's device buffer; host memory gets the planes through the handle's buffer
-    uint32_t *dst = nullptr;
+    T *dst = nullptr;
     if (out) {
         cudaPointerAttributes a;
         CK(cudaPointerGetAttributes(&a, out));
@@ -931,25 +931,25 @@ static int col_planes(b200_engine *e, const char *what, const char *buf, int pla
         } else if (a.type == cudaMemoryTypeManaged) dst = out;
     }
     const size_t words = (size_t)e->n_files * (size_t)planes * (size_t)n;
-    if (!dst) { ENSURE(cnt, words); dst = e->cnt; }
+    if (!dst) { ENSURE(cnt, words * sizeof(T) / sizeof(uint32_t)); dst = reinterpret_cast<T *>(e->cnt); }
     const int64_t warps = (int64_t)e->n_files * ((n + 31) / 32);
-    if (deep) CK(cudaMemsetAsync(deep, 0, 8, e->stream));
+    if (flag) CK(cudaMemsetAsync(flag, 0, 8, e->stream));
     CK(cudaEventRecord(e->ev0, e->stream));
     launch(nblk(warps, CNT_WARPS), v, (int32_t)((n + 31) / 32), dst); e->launches++;
     CK(cudaEventRecord(e->ev1, e->stream));
-    if (out && dst != out) CK(cudaMemcpyAsync(out, dst, words * 4, cudaMemcpyDeviceToHost, e->stream));
-    unsigned long long h_deep = 0;
-    if (deep) CK(cudaMemcpyAsync(&h_deep, deep, 8, cudaMemcpyDeviceToHost, e->stream));
+    if (out && dst != out) CK(cudaMemcpyAsync(out, dst, words * sizeof(T), cudaMemcpyDeviceToHost, e->stream));
+    unsigned long long h_flag = 0;
+    if (flag) CK(cudaMemcpyAsync(&h_flag, flag, 8, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     CK(cudaGetLastError());
-    if (h_deep) { snprintf(e->err, sizeof e->err, "a column has more than %u reads: its %s would not fit in 32 bits", QS_MAX_DEPTH, what); return -1; }
+    if (h_flag) { snprintf(e->err, sizeof e->err, "%s", flag_msg); return -1; }
     float ms = 0; cudaEventElapsedTime(&ms, e->ev0, e->ev1); e->last_kernel_ms = ms;
     return 0;
 }
 
 extern "C" int b200_mpileup_counts(b200_engine_t *e, int32_t min_baseQ, uint32_t *out, size_t cap_cols, int64_t *n_cols)
 {
-    return col_planes(e, "counts", "count", CNT_PLANES, out, cap_cols, n_cols, nullptr, [&](int blocks, const View &v, int32_t n_groups, uint32_t *dst) {
+    return col_planes(e, "counts", "count", CNT_PLANES, out, cap_cols, n_cols, nullptr, nullptr, [&](int blocks, const View &v, int32_t n_groups, uint32_t *dst) {
         k_mp_counts<<<blocks, CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, dst);
     });
 }
@@ -957,8 +957,19 @@ extern "C" int b200_mpileup_counts(b200_engine_t *e, int32_t min_baseQ, uint32_t
 extern "C" int b200_mpileup_qsums(b200_engine_t *e, int32_t min_baseQ, uint32_t *out, size_t cap_cols, int64_t *n_cols)
 {
     unsigned long long *deep = e ? e->d_misc + MISC_QSUM_DEEP : nullptr;
-    return col_planes(e, "quality sums", "quality sum", QS_PLANES, out, cap_cols, n_cols, deep, [&](int blocks, const View &v, int32_t n_groups, uint32_t *dst) {
+    char msg[96];
+    snprintf(msg, sizeof msg, "a column has more than %u reads: its quality sums would not fit in 32 bits", QS_MAX_DEPTH);
+    return col_planes(e, "quality sums", "quality sum", QS_PLANES, out, cap_cols, n_cols, deep, msg, [&](int blocks, const View &v, int32_t n_groups, uint32_t *dst) {
         k_mp_qsums<<<blocks, CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, dst, deep);
+    });
+}
+
+extern "C" int b200_mpileup_psums(b200_engine_t *e, int32_t min_baseQ, int64_t *out, size_t cap_cols, int64_t *n_cols)
+{
+    unsigned long long *ovf = e ? e->d_misc + MISC_PSUM_OVF : nullptr;
+    return col_planes(e, "position sums", "position sum", PS_PLANES, out, cap_cols, n_cols, ovf,
+                      "a column's sum of squared read positions would exceed 2^63 - 1", [&](int blocks, const View &v, int32_t n_groups, int64_t *dst) {
+        k_mp_psums<<<blocks, CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, dst, ovf);
     });
 }
 
@@ -1063,7 +1074,12 @@ extern "C" int b200_fetch_indels(b200_engine_t *e, b200_indel_t *alleles, size_t
     return 0;
 }
 
-extern "C" int b200_indel_qsums(b200_engine_t *e, b200_indel_qsum_t *out, size_t cap_rows)
+// The rows of b200_indel_qsums and b200_indel_psums beside the last indel table: checks, the row buffer (the handle's DBUF
+// `rows` with its capacity `cap`), the kernel (launch(blocks, view, flag): k_ind_qsums or k_ind_psums over the table's events) and the copy out.
+// flag: the d_misc slot where the kernel flags a sum it could not keep exact; the call then fails with flag_msg.
+template <class Row, class Launch>
+static int ind_sums(b200_engine *e, Row *out, size_t cap_rows, const char *buf, Row *b200_engine::*rows, size_t b200_engine::*cap, int flag_slot,
+                    const char *flag_msg, Launch launch)
 {
     if (!e || !e->staged || !e->ind_ready) {
         if (e) snprintf(e->err, sizeof e->err, "no indel table: call b200_mpileup_indels on the staged batch first");
@@ -1071,27 +1087,46 @@ extern "C" int b200_indel_qsums(b200_engine_t *e, b200_indel_qsum_t *out, size_t
     }
     CK(cudaSetDevice(e->device));
     e->last_kernel_ms = 0;
-    if (out && cap_rows < (size_t)e->ind_n) { snprintf(e->err, sizeof e->err, "quality sum buffer too small: need %lld rows", (long long)e->ind_n); return -2; }
-    if (out && e->ind_n && check_dst(e, out, "quality sum")) return -1;
+    if (out && cap_rows < (size_t)e->ind_n) { snprintf(e->err, sizeof e->err, "%s buffer too small: need %lld rows", buf, (long long)e->ind_n); return -2; }
+    if (out && e->ind_n && check_dst(e, out, buf)) return -1;
     if (e->ind_n == 0) return 0;
     // the events, hash slots, allele indices and rows of the table are still those b200_mpileup_indels left in HBM
-    ENSURE(ind_qs, (size_t)e->ind_n);
+    if (ensure(e, e->*rows, e->*cap, (size_t)e->ind_n)) return -1;
     View v; fill_view(e, v, nullptr, nullptr, 0, 0, 1);
-    unsigned long long *deep = e->d_misc + MISC_QSUM_DEEP;
+    unsigned long long *flag = e->d_misc + flag_slot;
     CK(cudaEventRecord(e->ev0, e->stream));
-    CK(cudaMemsetAsync(e->ind_qs, 0, (size_t)e->ind_n * sizeof(b200_indel_qsum_t), e->stream));
-    CK(cudaMemsetAsync(deep, 0, 8, e->stream));
-    k_ind_qsums<<<nblk(e->ind_nev, 256), 256, 0, e->stream>>>(v, (const IndelEv *)e->ind_ev, e->ind_nev, e->ind_tbl, e->ind_slot, e->ind_aidx,
-                                                            e->ind_tab, e->ind_qs, deep); e->launches++;
+    CK(cudaMemsetAsync(e->*rows, 0, (size_t)e->ind_n * sizeof(Row), e->stream));
+    CK(cudaMemsetAsync(flag, 0, 8, e->stream));
+    launch(nblk(e->ind_nev, 256), v, flag); e->launches++;
     CK(cudaEventRecord(e->ev1, e->stream));
-    if (out) CK(cudaMemcpyAsync(out, e->ind_qs, (size_t)e->ind_n * sizeof(b200_indel_qsum_t), cudaMemcpyDefault, e->stream));
-    unsigned long long h_deep = 0;
-    CK(cudaMemcpyAsync(&h_deep, deep, 8, cudaMemcpyDeviceToHost, e->stream));
+    if (out) CK(cudaMemcpyAsync(out, e->*rows, (size_t)e->ind_n * sizeof(Row), cudaMemcpyDefault, e->stream));
+    unsigned long long h_flag = 0;
+    CK(cudaMemcpyAsync(&h_flag, flag, 8, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     CK(cudaGetLastError());
-    if (h_deep) { snprintf(e->err, sizeof e->err, "an indel allele has more than %u entries on one strand: its quality sums would not fit in 32 bits", QS_MAX_DEPTH); return -1; }
+    if (h_flag) { snprintf(e->err, sizeof e->err, "%s", flag_msg); return -1; }
     float ms = 0; cudaEventElapsedTime(&ms, e->ev0, e->ev1); e->last_kernel_ms = ms;
     return 0;
+}
+
+extern "C" int b200_indel_qsums(b200_engine_t *e, b200_indel_qsum_t *out, size_t cap_rows)
+{
+    char msg[128];
+    snprintf(msg, sizeof msg, "an indel allele has more than %u entries on one strand: its quality sums would not fit in 32 bits", QS_MAX_DEPTH);
+    return ind_sums(e, out, cap_rows, "quality sum", &b200_engine::ind_qs, &b200_engine::cap_ind_qs, MISC_QSUM_DEEP, msg,
+                    [&](int blocks, const View &v, unsigned long long *deep) {
+        k_ind_qsums<<<blocks, 256, 0, e->stream>>>(v, (const IndelEv *)e->ind_ev, e->ind_nev, e->ind_tbl, e->ind_slot, e->ind_aidx,
+                                                   e->ind_tab, e->ind_qs, deep);
+    });
+}
+
+extern "C" int b200_indel_psums(b200_engine_t *e, b200_indel_psum_t *out, size_t cap_rows)
+{
+    return ind_sums(e, out, cap_rows, "position sum", &b200_engine::ind_ps, &b200_engine::cap_ind_ps, MISC_PSUM_OVF,
+                    "an indel allele's sum of squared read positions would exceed 2^63 - 1", [&](int blocks, const View &v, unsigned long long *ovf) {
+        k_ind_psums<<<blocks, 256, 0, e->stream>>>(v, (const IndelEv *)e->ind_ev, e->ind_nev, e->ind_tbl, e->ind_slot, e->ind_aidx,
+                                                   e->ind_ps, ovf);
+    });
 }
 
 extern "C" int b200_depth_text(b200_engine_t *e, const b200_depth_conf_t *c, char *out, size_t out_cap, size_t *out_len)

@@ -1,8 +1,8 @@
 // cli.cpp -- `b200samtools mpileup|depth|coverage|bedcov|gl`: the reference's CLI surface
 // for the pileup hot path, driving the CUDA engine through its C ABI; `counts` prints the
 // per-column base and indel counts of mpileup's rows, `indels` the indel alleles of its
-// columns (both with --qsums: their base-quality and mapq sums); `index` writes the BAI /
-// CSI those commands read a region through.
+// columns (both with --qsums: their base-quality and mapq sums, with --psums: their read-position
+// sums); `index` writes the BAI / CSI those commands read a region through.
 //
 // Option surfaces follow bam_plcmd.c:1096-1223 (mpileup), bam2depth.c:757-882
 // (depth) and coverage.c:343-424 (coverage), SURVEY.md Appendix B.  What stays
@@ -37,14 +37,16 @@
 
 using namespace b200;
 
-// The count, indel and quality-sum outputs are optional parts of an engine build: the CLI links against any implementation of
-// the C ABI (the CUDA library, or a CPU debug build of the column code that may not provide them), and `counts` / `indels`
-// (or their --qsums) refuse to run on one without theirs.
+// The count, indel, quality-sum and position-sum outputs are optional parts of an engine build: the CLI links against any
+// implementation of the C ABI (the CUDA library, or a CPU debug build of the column code that may not provide them), and
+// `counts` / `indels` (or their --qsums / --psums) refuse to run on one without theirs.
 #pragma weak b200_mpileup_counts
 #pragma weak b200_mpileup_indels
 #pragma weak b200_fetch_indels
 #pragma weak b200_mpileup_qsums
 #pragma weak b200_indel_qsums
+#pragma weak b200_mpileup_psums
+#pragma weak b200_indel_psums
 
 namespace {
 
@@ -139,6 +141,7 @@ struct WinWorker {
     std::vector<uint32_t> cnt;   // count planes of the window (counts)
     std::vector<b200_indel_t> ind; std::string ind_seq;   // indel table of the window (indels)
     std::vector<uint32_t> qs; std::vector<b200_indel_qsum_t> ind_qs;   // quality sums of the window (--qsums)
+    std::vector<int64_t> ps; std::vector<b200_indel_psum_t> ind_ps;    // position sums of the window (--psums)
     void rewind() { std::fill(cursor.begin(), cursor.end(), 0); }
     int fail(const char *tool) { rc = -1; err = std::string("samtools ") + tool + ": " + b200_last_error(eng.e); return -1; }
 };
@@ -321,6 +324,7 @@ struct MpOpts {
     bool counts = false;   // `counts`: the rows of mpileup as per-column counts (b200_mpileup_counts)
     bool indels = false;   // `indels`: the indel alleles of mpileup's columns (b200_mpileup_indels)
     bool qsums = false;    // --qsums: `counts` / `indels` add the quality sums (b200_mpileup_qsums / b200_indel_qsums)
+    bool psums = false;    // --psums: `counts` / `indels` add the BP-5 sums (b200_mpileup_psums / b200_indel_psums), after any --qsums
     // host columns (bam_plcmd.c:727-855): record fields in the order of the MPLP_PRINT_* bits, then aux tags in the order given
     std::vector<std::string> xcols;      // "QNAME" "FLAG" "RNAME" "POS" "MAPQ" "RNEXT" "PNEXT" "RLEN" or a two-letter tag
     int n_xfields = 0;                   // how many of them are record fields (joined with ','; tags use x_sep)
@@ -541,6 +545,11 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn, const std::vector
                     w.qs.resize((size_t)nfn * B200_QSUM_PLANES * cap + 1);
                     if (b200_mpileup_qsums(w.eng.e, o.min_baseQ, w.qs.data(), cap, &n) != 0) { w.fail("counts"); return; }
                 }
+                const int np = o.psums ? B200_PSUM_PLANES : 0;
+                if (o.psums) {
+                    w.ps.resize((size_t)nfn * B200_PSUM_PLANES * cap + 1);
+                    if (b200_mpileup_psums(w.eng.e, o.min_baseQ, w.ps.data(), cap, &n) != 0) { w.fail("counts"); return; }
+                }
                 const int64_t n_all = std::min(we, h.lens[(size_t)tid]) - wb;
                 for (int64_t c = 0; c < n; ++c) {
                     bool any = false;
@@ -549,12 +558,13 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn, const std::vector
                     const int64_t p = wb + c;
                     if (o.bed && !o.bed->overlap(name, p, p + 1)) continue;
                     appendf(w, "%s\t%lld\t%c", name.c_str(), (long long)p + 1, (ref && p < (int64_t)ref->size()) ? (*ref)[(size_t)p] : 'N');
-                    const size_t need = w.need + (size_t)nfn * (B200_COUNT_PLANES + nq) * 11 + 2;
+                    const size_t need = w.need + (size_t)nfn * ((B200_COUNT_PLANES + nq) * 11 + np * 21) + 2;
                     if (w.out.size() < need) w.out.resize(std::max(2 * w.out.size(), need));
                     char *q = w.out.data() + w.need;
                     for (int f = 0; f < nfn; ++f) {
                         for (int k = 0; k < B200_COUNT_PLANES; ++k) { *q++ = '\t'; q = std::to_chars(q, w.out.data() + w.out.size(), w.cnt[((size_t)f * B200_COUNT_PLANES + (size_t)k) * plane + (size_t)c]).ptr; }
                         for (int k = 0; k < nq; ++k) { *q++ = '\t'; q = std::to_chars(q, w.out.data() + w.out.size(), w.qs[((size_t)f * B200_QSUM_PLANES + (size_t)k) * plane + (size_t)c]).ptr; }
+                        for (int k = 0; k < np; ++k) { *q++ = '\t'; q = std::to_chars(q, w.out.data() + w.out.size(), w.ps[((size_t)f * B200_PSUM_PLANES + (size_t)k) * plane + (size_t)c]).ptr; }
                     }
                     *q++ = '\n';
                     w.need = (size_t)(q - w.out.data());
@@ -571,6 +581,10 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn, const std::vector
                 if (o.qsums) {   // then bq_fwd bq_rev mq_fwd mq_rev mq0_fwd mq0_rev
                     w.ind_qs.resize((size_t)na + 1);
                     if (b200_indel_qsums(w.eng.e, w.ind_qs.data(), w.ind_qs.size()) != 0) { w.fail("indels"); return; }
+                }
+                if (o.psums) {   // then bp5_fwd bp5_rev bp5sq_fwd bp5sq_rev
+                    w.ind_ps.resize((size_t)na + 1);
+                    if (b200_indel_psums(w.eng.e, w.ind_ps.data(), w.ind_ps.size()) != 0) { w.fail("indels"); return; }
                 }
                 std::string tok;
                 for (int64_t k = 0; k < na; ++k) {
@@ -589,6 +603,10 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn, const std::vector
                     if (o.qsums) {
                         const b200_indel_qsum_t &x = w.ind_qs[(size_t)k];
                         appendf(w, "\t%u\t%u\t%u\t%u\t%u\t%u", x.bq_fwd, x.bq_rev, x.mq_fwd, x.mq_rev, x.mq0_fwd, x.mq0_rev);
+                    }
+                    if (o.psums) {
+                        const b200_indel_psum_t &x = w.ind_ps[(size_t)k];
+                        appendf(w, "\t%lld\t%lld\t%lld\t%lld", (long long)x.bp5_fwd, (long long)x.bp5_rev, (long long)x.bp5sq_fwd, (long long)x.bp5sq_rev);
                     }
                     appendf(w, "\n");
                 }
@@ -651,7 +669,7 @@ int main_mpileup(int argc, char **argv, MpCmd cmd)
         {"output-mods", 0, 0, 'M'}, {"output-BP", 0, 0, 'O'}, {"output-bp", 0, 0, 'O'}, {"output-BP-5", 0, 0, 14}, {"output-bp-5", 0, 0, 14},
         {"output-MQ", 0, 0, 's'}, {"output-mq", 0, 0, 's'}, {"customized-index", 0, 0, 'X'}, {"reverse-del", 0, 0, 6},
         {"output-extra", 1, 0, 7}, {"output-sep", 1, 0, 8}, {"output-empty", 1, 0, 9}, {"no-output-ins", 0, 0, 10},
-        {"no-output-ins-mods", 0, 0, 11}, {"no-output-del", 0, 0, 12}, {"no-output-ends", 0, 0, 13}, {"qsums", 0, 0, 15}, {0, 0, 0, 0} };
+        {"no-output-ins-mods", 0, 0, 11}, {"no-output-del", 0, 0, 12}, {"no-output-ends", 0, 0, 13}, {"qsums", 0, 0, 15}, {"psums", 0, 0, 16}, {0, 0, 0, 0} };
     int c;
     optind = 1;
     while ((c = getopt_long(argc, argv, "Af:r:l:q:Q:RC:Bd:b:o:EG:6OsxXaM", lo, nullptr)) >= 0) {
@@ -659,7 +677,7 @@ int main_mpileup(int argc, char **argv, MpCmd cmd)
             char opt[3] = {'-', (char)c, 0};
             fprintf(stderr, "b200samtools %s: %s is an option of the pileup text\n\n"
                             "Usage: b200samtools %s [-f ref.fa] [-r reg] [-l bed] [-b list] [-X] [-q INT] [-Q INT] [-B] [-E] [-C INT] [-d INT]\n"
-                            "                           [-x] [-A] [-6] [-G file] [-R] [--rf FLAGS] [--ff FLAGS] [-a[a]] [-o out] [--qsums]\n"
+                            "                           [-x] [-A] [-6] [-G file] [-R] [--rf FLAGS] [--ff FLAGS] [-a[a]] [-o out] [--qsums] [--psums]\n"
                             "                           in1.bam [in2.bam ...]\n",
                     tool, c < 32 ? argv[optind - 1] : opt, tool);
             return 1;
@@ -700,6 +718,9 @@ int main_mpileup(int argc, char **argv, MpCmd cmd)
         case 15:
             if (!o.counts && !o.indels) { fprintf(stderr, "b200samtools mpileup: --qsums is an option of `counts` and `indels`\n"); return 1; }
             o.qsums = true; break;
+        case 16:
+            if (!o.counts && !o.indels) { fprintf(stderr, "b200samtools mpileup: --psums is an option of `counts` and `indels`\n"); return 1; }
+            o.psums = true; break;
         case 'f': o.fa = Fasta::load(optarg); if (!o.fa) { fprintf(stderr, "[E::fai_load] failed to open %s\n", optarg); return 1; } o.fa_fn = optarg; break;
         case 'd': o.max_depth = atoi(optarg); break;
         case 'r': o.reg = optarg; break;
@@ -729,6 +750,7 @@ int main_mpileup(int argc, char **argv, MpCmd cmd)
     if (o.counts && !b200_mpileup_counts) { fprintf(stderr, "b200samtools counts: this engine build has no count output\n"); return 1; }
     if (o.indels && (!b200_mpileup_indels || !b200_fetch_indels)) { fprintf(stderr, "b200samtools indels: this engine build has no indel output\n"); return 1; }
     if (o.qsums && (o.counts ? !b200_mpileup_qsums : !b200_indel_qsums)) { fprintf(stderr, "b200samtools %s: this engine build has no quality sums\n", tool); return 1; }
+    if (o.psums && (o.counts ? !b200_mpileup_psums : !b200_indel_psums)) { fprintf(stderr, "b200samtools %s: this engine build has no position sums\n", tool); return 1; }
     if (!o.realn && o.redo_baq) { fprintf(stderr, "Error: The -B option cannot be combined with -E\n"); return 1; }
     if (use_orphan) o.no_orphan = false;
     {   // record fields print in the order of the MPLP_PRINT_* bits (bam_plcmd.c:185-196,728-795), tags after them in the order given

@@ -1,5 +1,5 @@
 // mpileup_indel.cuh -- per-column indel alleles of the mpileup column stage (b200_mpileup_indels / b200_fetch_indels) and
-// their quality sums (b200_indel_qsums).
+// their quality and read-position sums (b200_indel_qsums, b200_indel_psums).
 // Included by engine.cu.
 //
 // The distinct "+n..." / "-n" tokens the text prints after the entries of one (column, file) that pass -Q, with strand-split
@@ -19,7 +19,8 @@
 //      filters.  A deep column of one shared allele costs one probe per event, not a pass over the allele list.
 //   6. k_ind_mark + two scans: an event that owns its slot starts an allele; allele index and symbol offset.
 //   7. k_ind_emit: the table rows and their symbols.
-// b200_indel_qsums runs k_ind_qsums later over the same events, which stay in HBM until the next stage.
+// b200_indel_qsums and b200_indel_psums run k_ind_qsums / k_ind_psums later over the same events, which stay in HBM until
+// the next stage.
 // Every event kernel is launched over the stage's bound on the events (ind_bounds) and reads the real count from HBM, so
 // the call synchronises with the host once, at the end.
 constexpr int IND_WARPS = 4;
@@ -153,11 +154,12 @@ __global__ void k_ind_emit(const IndelEv *ev, const uint32_t *n_ev, uint32_t cap
     for (int32_t i = 0; i < x.len; ++i) seq[a_seq[j] + (uint64_t)i] = src[i];
 }
 
-// b200_indel_qsums: thread per event of the table.  The allele's row is the row of its slot's owner (the first appearance,
-// k_ind_insert); the event adds its entry's BQ / MQ / MQ0 (plp_core.h mp_entry_qs) on its strand.  qs: the rows, zeroed by
-// the caller.  deep: set where an allele has more than QS_MAX_DEPTH entries on one strand (a sum could wrap).
-__global__ void k_ind_qsums(View v, const IndelEv *ev, uint32_t n_ev, const int32_t *tbl, const uint32_t *slot, const uint32_t *a_idx,
-                            const b200_indel_t *tab, b200_indel_qsum_t *qs, unsigned long long *deep)
+// b200_indel_qsums / b200_indel_psums: thread per event of the table.  The allele's row is the row of its slot's owner (the
+// first appearance, k_ind_insert); add(x, d, e, row, owner) adds what the event's entry contributes: e is the cursor of the
+// entry the token follows, with the query position and is_del bit the walk kept in the event.
+template <class Add>
+__device__ __forceinline__ void ind_event_sums(const View &v, const IndelEv *ev, uint32_t n_ev, const int32_t *tbl, const uint32_t *slot,
+                                               const uint32_t *a_idx, Add add)
 {
     const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= n_ev) return;
@@ -165,9 +167,32 @@ __global__ void k_ind_qsums(View v, const IndelEv *ev, uint32_t n_ev, const int3
     const int32_t owner = tbl[2 * (size_t)x.lo + slot[j]];
     const uint32_t row = a_idx[owner];
     const ReadDesc d = load_desc(v.desc + x.read);
-    Ent e; e.qpos = x.qpos;                                  // all ent_qual reads of the cursor
-    const EntQs q = mp_entry_qs(ent_qual(v, d, e), d);
-    uint32_t *o = reinterpret_cast<uint32_t *>(qs + row) + (x.fl & 1u);
-    atomicAdd(o, q.bq); atomicAdd(o + 2, q.mq); atomicAdd(o + 4, q.mq0);
-    if (owner == (int32_t)j && (tab[row].fwd > QS_MAX_DEPTH || tab[row].rev > QS_MAX_DEPTH)) *deep = 1ull;
+    Ent e; e.qpos = x.qpos; e.is_del = (uint8_t)((x.fl >> 1) & 1u);   // all ent_qual and qpos5_of read of the cursor
+    add(x, d, e, row, owner == (int32_t)j);
+}
+
+// the event adds its entry's BQ / MQ / MQ0 (plp_core.h mp_entry_qs) on its strand.  qs: the rows, zeroed by the caller.
+// deep: set where an allele has more than QS_MAX_DEPTH entries on one strand (a sum could wrap).
+__global__ void k_ind_qsums(View v, const IndelEv *ev, uint32_t n_ev, const int32_t *tbl, const uint32_t *slot, const uint32_t *a_idx,
+                            const b200_indel_t *tab, b200_indel_qsum_t *qs, unsigned long long *deep)
+{
+    ind_event_sums(v, ev, n_ev, tbl, slot, a_idx, [&](const IndelEv &x, const ReadDesc &d, const Ent &e, uint32_t row, bool owner) {
+        const EntQs q = mp_entry_qs(ent_qual(v, d, e), d);
+        uint32_t *o = reinterpret_cast<uint32_t *>(qs + row) + (x.fl & 1u);
+        atomicAdd(o, q.bq); atomicAdd(o + 2, q.mq); atomicAdd(o + 4, q.mq0);
+        if (owner && (tab[row].fwd > QS_MAX_DEPTH || tab[row].rev > QS_MAX_DEPTH)) *deep = 1ull;
+    });
+}
+
+// the event adds its entry's BP-5 and its square (plp_core.h mp_entry_ps) on its strand.  ps: the rows, zeroed by the caller.
+// ovf: set where a sum of squares would exceed INT64_MAX (ps_sq_over on the value the atomicAdd found).
+__global__ void k_ind_psums(View v, const IndelEv *ev, uint32_t n_ev, const int32_t *tbl, const uint32_t *slot, const uint32_t *a_idx,
+                            b200_indel_psum_t *ps, unsigned long long *ovf)
+{
+    ind_event_sums(v, ev, n_ev, tbl, slot, a_idx, [&](const IndelEv &x, const ReadDesc &d, const Ent &e, uint32_t row, bool) {
+        const EntPs p = mp_entry_ps(d, e);
+        unsigned long long *o = reinterpret_cast<unsigned long long *>(ps + row) + (x.fl & 1u);
+        atomicAdd(o, (unsigned long long)p.bp5);              // two's complement: the signed sum
+        if (ps_sq_over(atomicAdd(o + 2, (unsigned long long)p.sq), p.sq)) *ovf = 1ull;
+    });
 }

@@ -460,6 +460,29 @@ PLP_HD EntQs mp_entry_qs(int q, const ReadDesc &d)
     return r;
 }
 
+// ---- per-column read-position sums of the entries (mpileup_cnt.cuh, mpileup_indel.cuh): what a parser of the BP-5 text adds --
+// Planes per file: the BP-5 sums of kinds 0-6 (mp_entry_channel & 15) of forward-strand entries, the same for reverse-strand
+// ones (+ PS_REV), then the sums of the squares (+ PS_SQ) in the same order.
+enum { PS_REV = 7, PS_SQ = 14, PS_PLANES = B200_PSUM_PLANES };
+// the "--output-BP-5" number of an entry (bam_plcmd.c:753-759): signed, <= 0 for a reverse-strand entry of a read without SEQ
+PLP_HD int32_t qpos5_of(const ReadDesc &d, const Ent &e)
+{
+    return (d.fl & RD_REV) ? d.l_qseq - e.qpos + (int)e.is_del : e.qpos + 1;
+}
+struct EntPs { int64_t bp5; uint64_t sq; };
+// an entry that passes -Q: its BP-5 and the square of it (|BP-5| < 2^31, so the square is below 2^62)
+PLP_HD EntPs mp_entry_ps(const ReadDesc &d, const Ent &e)
+{
+    EntPs r;
+    r.bp5 = qpos5_of(d, e);
+    r.sq = (uint64_t)(r.bp5 * r.bp5);
+    return r;
+}
+// the checked add of a sum of squares: true where old + x exceeds INT64_MAX.  Exact as long as old itself is at most
+// INT64_MAX (the first add that is not raises the flag), since x < 2^62 then keeps the unsigned add from wrapping; so it
+// holds for a lane-private cell and for the old value an atomicAdd returns alike.
+PLP_HD bool ps_sq_over(uint64_t old, uint64_t x) { return old + x > (uint64_t)INT64_MAX; }
+
 // ---- indel alleles of the entries (mpileup_indel.cuh): the distinct "+n..." / "-n" tokens of one (column, file) ---------
 // An allele is its signed length (>= 0: an insertion of that many symbols, forward-strand form from ins_symbols; < 0: a
 // deletion of -len reference bases, which name it by length alone) and, for an insertion, the symbol bytes.  Two tokens are
@@ -490,11 +513,6 @@ struct MpFileSz {
     int32_t nplp, cnt;
     uint32_t seq_len, bp_len, bp5_len;
 };
-
-PLP_HD int32_t qpos5_of(const ReadDesc &d, const Ent &e)
-{
-    return (d.fl & RD_REV) ? d.l_qseq - e.qpos + (int)e.is_del : e.qpos + 1;
-}
 
 // quality the reference tests against -Q for read d at column c (simple reads without the cursor)
 PLP_HD int col_qual(const View &v, const ReadDesc &d, int32_t i, int32_t c)

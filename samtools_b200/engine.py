@@ -21,11 +21,21 @@ EXPORTS = ['b200_engine_create', 'b200_engine_destroy', 'b200_last_error', 'b200
            'b200_fetch_mapq_keep', 'b200_pileup_entries', 'b200_last_kernel_ms', 'b200_last_stage_ms', 'b200_set_keep_raw', 'b200_restage', 'b200_last_stage_device_ms',
            'b200_launch_count', 'b200_last_mpileup_parts_ms', 'b200_gl_rng_draws', 'b200_last_baq_ms',
            'b200_errmod_cal', 'b200_glfgen', 'b200_cap_mapq', 'b200_mpileup_text_bound', 'b200_depth_text_bound', 'b200_bedcov',
-           'b200_mpileup_counts', 'b200_mpileup_indels', 'b200_fetch_indels', 'b200_mpileup_qsums', 'b200_indel_qsums']
+           'b200_mpileup_counts', 'b200_mpileup_indels', 'b200_fetch_indels', 'b200_mpileup_qsums', 'b200_indel_qsums',
+           'b200_mpileup_psums', 'b200_indel_psums']
 COUNT_PLANES = 19   # b200_mpileup_counts: per file A C G T N del skip +ins -del, forward then reverse strand, then n_plp
 QSUM_PLANES = 42    # b200_mpileup_qsums: per file BQ sums, MQ sums, MQ0 counts, each of A C G T N del skip, forward then reverse
 # b200_indel_qsum_t, one row of b200_indel_qsums beside the row of b200_mpileup_indels
 INDEL_QSUM_FIELDS = ('bq_fwd', 'bq_rev', 'mq_fwd', 'mq_rev', 'mq0_fwd', 'mq0_rev')
+PSUM_PLANES = 28    # b200_mpileup_psums: per file BP-5 sums, sums of BP-5 squared, each of A C G T N del skip, forward then reverse
+
+
+class IndelPsum(C.Structure):
+    """b200_indel_psum_t, one row of b200_indel_psums beside the row of b200_mpileup_indels"""
+    _fields_ = [('bp5_fwd', C.c_int64), ('bp5_rev', C.c_int64), ('bp5sq_fwd', C.c_int64), ('bp5sq_rev', C.c_int64)]
+
+
+INDEL_PSUM_FIELDS = tuple(f for f, _ in IndelPsum._fields_)
 # b200_indel_t, one row of b200_mpileup_indels: len >= 0 an insertion of len symbols at seq[seq_off:], < 0 a deletion of -len
 INDEL_DTYPE = np.dtype([('col', '<i4'), ('file', '<i4'), ('len', '<i4'), ('fwd', '<u4'), ('rev', '<u4'), ('pad', '<u4'),
                         ('seq_off', '<u8')])
@@ -102,6 +112,8 @@ def load_library():
         lib.b200_fetch_indels.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
         lib.b200_mpileup_qsums.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64)]
         lib.b200_indel_qsums.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+        lib.b200_mpileup_psums.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64)]
+        lib.b200_indel_psums.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_fetch_qual.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_fetch_mapq_keep.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_pileup_entries.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -250,17 +262,17 @@ class Engine:
         k = n.value
         return pos[:k], nb[:k * n_files].reshape(k, n_files), qs[:k * n_files * 4].reshape(k, n_files, 4), p25[:k * n_files * 25].reshape(k, n_files, 25)
 
-    def _planes(self, fn, planes, min_baseQ, out):
+    def _planes(self, fn, planes, min_baseQ, out, np_dtype=np.uint32, torch_dtype='int32'):
         n = C.c_int64(0)
         shape = (self._n_files, planes, self._n_cols)     # the stage's n_cols are the columns of the planes
         if out is None:
-            a = np.zeros(shape, np.uint32)
+            a = np.zeros(shape, np_dtype)
             if getattr(self.lib, fn)(self.h, min_baseQ, _ptr(a), shape[2], C.byref(n)) != 0:
                 self._err(fn)
             return a
         import torch
-        if out.dtype != torch.int32 or not out.is_cuda or not out.is_contiguous() or out.device.index != self.device:
-            raise ValueError(f'out must be a contiguous torch.int32 tensor on cuda:{self.device}')
+        if out.dtype != getattr(torch, torch_dtype) or not out.is_cuda or not out.is_contiguous() or out.device.index != self.device:
+            raise ValueError(f'out must be a contiguous torch.{torch_dtype} tensor on cuda:{self.device}')
         if tuple(out.shape) != shape:
             raise ValueError(f'out must have shape {list(shape)}')
         torch.cuda.current_stream(out.device).synchronize()   # the engine writes on its own stream
@@ -279,6 +291,12 @@ class Engine:
         sums, MQ sums and MQ0 counts (plane s * 14 + strand * 7 + kind), or, given `out`, a contiguous torch.int32 CUDA
         tensor of that shape on the handle's device, filled in place on the device (and returned)."""
         return self._planes('b200_mpileup_qsums', QSUM_PLANES, min_baseQ, out)
+
+    def mpileup_psums(self, min_baseQ=13, out=None):
+        """Per-column read-position sums of the staged window (b200_mpileup_psums): a numpy int64 [n_files, 28, n] array of
+        BP-5 sums and sums of BP-5 squared (plane s * 14 + strand * 7 + kind), or, given `out`, a contiguous torch.int64 CUDA
+        tensor of that shape on the handle's device, filled in place on the device (and returned)."""
+        return self._planes('b200_mpileup_psums', PSUM_PLANES, min_baseQ, out, np.int64, 'int64')
 
     def mpileup_indels(self, min_baseQ=13, device=False):
         """Per-column indel alleles of the staged window (b200_mpileup_indels): (rows, symbols).  By default a numpy structured
@@ -305,23 +323,32 @@ class Engine:
             self._err('b200_fetch_indels')
         return rows, seq
 
+    def _allele_rows(self, fn, width, np_dtype, torch_dtype, device):
+        n = self._n_alleles
+        if not device:
+            a = np.zeros((n, width), np_dtype)
+            if getattr(self.lib, fn)(self.h, _ptr(a) if n else None, n) != 0:
+                self._err(fn)
+            return a
+        import torch
+        dev = torch.device('cuda', self.device)
+        t = torch.empty((n, width), dtype=getattr(torch, torch_dtype), device=dev)
+        torch.cuda.current_stream(dev).synchronize()   # the engine writes on its own stream
+        if getattr(self.lib, fn)(self.h, C.c_void_p(t.data_ptr()) if n else None, n) != 0:
+            self._err(fn)
+        return t
+
     def indel_qsums(self, device=False):
         """Quality sums of the rows of the last mpileup_indels on the staged batch (b200_indel_qsums), one row per allele in
         the table's order, columns INDEL_QSUM_FIELDS: a numpy uint32 [n, 6] array, or with device=True an int32 [n, 6] CUDA
         tensor on the handle's device, filled on the device."""
-        n = self._n_alleles
-        if not device:
-            a = np.zeros((n, len(INDEL_QSUM_FIELDS)), np.uint32)
-            if self.lib.b200_indel_qsums(self.h, _ptr(a) if n else None, n) != 0:
-                self._err('b200_indel_qsums')
-            return a
-        import torch
-        dev = torch.device('cuda', self.device)
-        t = torch.empty((n, len(INDEL_QSUM_FIELDS)), dtype=torch.int32, device=dev)
-        torch.cuda.current_stream(dev).synchronize()   # the engine writes on its own stream
-        if self.lib.b200_indel_qsums(self.h, C.c_void_p(t.data_ptr()) if n else None, n) != 0:
-            self._err('b200_indel_qsums')
-        return t
+        return self._allele_rows('b200_indel_qsums', len(INDEL_QSUM_FIELDS), np.uint32, 'int32', device)
+
+    def indel_psums(self, device=False):
+        """Read-position sums of the rows of the last mpileup_indels on the staged batch (b200_indel_psums), one row per
+        allele in the table's order, columns INDEL_PSUM_FIELDS (the IndelPsum row): a numpy int64 [n, 4] array, or with
+        device=True an int64 [n, 4] CUDA tensor on the handle's device, filled on the device."""
+        return self._allele_rows('b200_indel_psums', len(INDEL_PSUM_FIELDS), np.int64, 'int64', device)
 
     def fetch_qual(self, nbytes):
         q = np.zeros(nbytes, np.uint8)
