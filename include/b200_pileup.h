@@ -30,6 +30,7 @@
  *   b200_indel_qsums()    (the same, per indel allele)     -> BQ / MQ sums and MQ0 counts of each allele's entries
  *   b200_mpileup_psums()  the --output-BP-5 column         bam_plcmd.c:753-759 -> per-column BP-5 sums and sums of squares
  *   b200_indel_psums()    (the same, per indel allele)     -> BP-5 sums and sums of squares of each allele's entries
+ *   b200_mpileup_ranksums() the -s, qual and BP-5 columns  -> per-column Mann-Whitney U of BQ / MQ / BP-5, ref vs alt bases
  *   b200_pileup_entries() bam_plp64_next/resolve_cigar2   (htslib sam.c) -> arrays of bam_pileup1_t fields
  *
  * Conventions: plain C, caller-owned host buffers, int return codes (0 ok,
@@ -301,6 +302,25 @@ typedef struct {
     int64_t bp5_fwd, bp5_rev, bp5sq_fwd, bp5sq_rev;
 } b200_indel_psum_t;
 int b200_indel_psums(b200_engine_t *e, b200_indel_psum_t *out, size_t cap_rows);
+/* per-column rank-sum bias statistics of the mpileup column stage, beside the counts: the Mann-Whitney U test of base
+ * quality, mapping quality and read position, reference against non-reference bases, as a parser of the
+ * `mpileup --reverse-del -s --output-BP-5` text would compute it over the entries that pass -Q (min_baseQ).  A class entry
+ * is an A, C, G or T entry (count planes r * 9 + 0..3): of the ref class where the text prints '.' / ',', of the alt class
+ * where it prints a letter (all non-reference bases pooled); deletions, skips and N / IUPAC bases take no part.  Its values
+ * are BQ and MQ as in b200_mpileup_qsums (0..93) and its BP-5 as in b200_mpileup_psums (>= 1), with a BP-5 above 1024
+ * ranked as 1024 (the cap is part of the definition: it keeps the work per column independent of the read length).
+ * Per file 8 int64 planes, laid out, sized and delivered exactly as those of b200_mpileup_counts:
+ * out[(f * 8 + k) * n + c]; out == NULL computes only; host or device memory; cap_cols < n returns -2; needs a batch staged
+ * in B200_MODE_MPILEUP.  Planes
+ *   0 n_ref,  1 n_alt,  2 / 3 U2 / T of BQ,  4 / 5 U2 / T of MQ,  6 / 7 U2 / T of BP-5
+ *   U2 = sum over (alt a, ref r) of 2 [a > r] + [a == r]    (twice the U of the alt sample)
+ *   T  = sum over values v of t_v^3 - t_v                    (t_v: ref and alt entries of value v; the tie term)
+ * planes 2-7 are 0 where a class is empty; n_ref + n_alt is the sum of count planes A C G T of both strands.  With
+ * N = n_ref + n_alt, U = U2 / 2 has mean n_ref n_alt / 2 and variance n_ref n_alt / 12 ((N + 1) - T / (N (N - 1))).  The
+ * planes are exact for N <= 2097151 (2^21 - 1); the call fails instead of wrapping on a deeper column.
+ * b200_last_kernel_ms() covers it. */
+#define B200_RANK_PLANES 8
+int b200_mpileup_ranksums(b200_engine_t *e, int32_t min_baseQ, int64_t *out, size_t cap_cols, int64_t *n_cols);
 /* htslib's per-column / per-read entry points on the device (tier T1 support; one column or one small batch per call):
  *   b200_errmod_cal   errmod_cal(em, n, m, bases, q) of htslib errmod.c (callers bam2bcf.c:121, phase.c:754, cut_target.c:84):
  *                     `bases` (q<<5|strand<<4|allele) is left sorted like the reference leaves it, q[m*m] receives the

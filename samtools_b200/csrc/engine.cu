@@ -254,6 +254,7 @@ __global__ void __launch_bounds__(TILE) k_mpileup_write(MpFmt fmt, const uint32_
 #include "mpileup_ent.cuh"
 #include "mpileup_cnt.cuh"
 #include "mpileup_indel.cuh"
+#include "mpileup_rank.cuh"
 
 struct DpFmt {
     View v; DpConf cf;
@@ -905,9 +906,10 @@ extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c,
     return text_end(e, e->col_off + nt, bound, out, out_cap, out_len);
 }
 
-// The planes of b200_mpileup_counts, b200_mpileup_qsums and b200_mpileup_psums: checks, destination, the kernel
-// (launch(blocks, view, n_groups, dst): k_mp_counts, k_mp_qsums or k_mp_psums), the copy to host memory.  T: the cell type.
-// flag: the d_misc slot where the kernel flags a sum it could not keep exact, or nullptr; the call then fails with flag_msg.
+// The planes of b200_mpileup_counts, b200_mpileup_qsums, b200_mpileup_psums and b200_mpileup_ranksums: checks,
+// destination, the kernels (launch(blocks, view, n_groups, dst), nonzero on an error: k_mp_counts, k_mp_qsums, k_mp_psums,
+// or the two phases of mpileup_rank.cuh), the copy to host memory.  T: the cell type.  flag: the d_misc slot where a kernel
+// flags a value it could not keep exact, or nullptr; the call then fails with flag_msg.
 template <class T, class Launch>
 static int col_planes(b200_engine *e, const char *what, const char *buf, int planes, T *out, size_t cap_cols, int64_t *n_cols,
                       unsigned long long *flag, const char *flag_msg, Launch launch)
@@ -935,7 +937,8 @@ static int col_planes(b200_engine *e, const char *what, const char *buf, int pla
     const int64_t warps = (int64_t)e->n_files * ((n + 31) / 32);
     if (flag) CK(cudaMemsetAsync(flag, 0, 8, e->stream));
     CK(cudaEventRecord(e->ev0, e->stream));
-    launch(nblk(warps, CNT_WARPS), v, (int32_t)((n + 31) / 32), dst); e->launches++;
+    if (launch(nblk(warps, CNT_WARPS), v, (int32_t)((n + 31) / 32), dst)) return -1;
+    e->launches++;
     CK(cudaEventRecord(e->ev1, e->stream));
     if (out && dst != out) CK(cudaMemcpyAsync(out, dst, words * sizeof(T), cudaMemcpyDeviceToHost, e->stream));
     unsigned long long h_flag = 0;
@@ -951,6 +954,7 @@ extern "C" int b200_mpileup_counts(b200_engine_t *e, int32_t min_baseQ, uint32_t
 {
     return col_planes(e, "counts", "count", CNT_PLANES, out, cap_cols, n_cols, nullptr, nullptr, [&](int blocks, const View &v, int32_t n_groups, uint32_t *dst) {
         k_mp_counts<<<blocks, CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, dst);
+        return 0;
     });
 }
 
@@ -961,6 +965,7 @@ extern "C" int b200_mpileup_qsums(b200_engine_t *e, int32_t min_baseQ, uint32_t 
     snprintf(msg, sizeof msg, "a column has more than %u reads: its quality sums would not fit in 32 bits", QS_MAX_DEPTH);
     return col_planes(e, "quality sums", "quality sum", QS_PLANES, out, cap_cols, n_cols, deep, msg, [&](int blocks, const View &v, int32_t n_groups, uint32_t *dst) {
         k_mp_qsums<<<blocks, CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, dst, deep);
+        return 0;
     });
 }
 
@@ -970,6 +975,25 @@ extern "C" int b200_mpileup_psums(b200_engine_t *e, int32_t min_baseQ, int64_t *
     return col_planes(e, "position sums", "position sum", PS_PLANES, out, cap_cols, n_cols, ovf,
                       "a column's sum of squared read positions would exceed 2^63 - 1", [&](int blocks, const View &v, int32_t n_groups, int64_t *dst) {
         k_mp_psums<<<blocks, CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, dst, ovf);
+        return 0;
+    });
+}
+
+extern "C" int b200_mpileup_ranksums(b200_engine_t *e, int32_t min_baseQ, int64_t *out, size_t cap_cols, int64_t *n_cols)
+{
+    unsigned long long *deep = e ? e->d_misc + MISC_RANK_DEEP : nullptr;
+    char msg[128];
+    snprintf(msg, sizeof msg, "a column has more than %u reference and non-reference bases: its rank sums would not fit in 64 bits", RS_MAX_DEPTH);
+    return col_planes(e, "rank sums", "rank sum", RS_PLANES, out, cap_cols, n_cols, deep, msg, [&](int blocks, const View &v, int32_t n_groups, int64_t *dst) {
+        // the list of active (file, column) pairs is sized by all of them; phase 2 reads its length from HBM
+        const int64_t pairs = (int64_t)e->n_files * v.ncols;
+        ENSURE(rk_act, (size_t)pairs); ENSURE(rk_off, (size_t)pairs + 1); ENSURE(rk_list, (size_t)pairs);
+        k_rank_counts<<<blocks, CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, dst, e->rk_act, deep);
+        if (launch_scan<ScanSum, 4, false>(e, e->rk_act, e->rk_off, pairs)) return -1;
+        k_rank_list<<<nblk(pairs, 256), 256, 0, e->stream>>>(e->rk_act, e->rk_off, pairs, e->rk_list); e->launches++;
+        const int hb = (int)std::min<int64_t>((int64_t)e->n_sm * RS_BLOCKS_PER_SM, nblk(pairs, RS_WARPS));
+        k_rank_hist<<<hb, RS_WARPS * 32, 0, e->stream>>>(v, min_baseQ, e->rk_list, e->rk_off + pairs, dst); e->launches++;
+        return 0;
     });
 }
 

@@ -42,7 +42,7 @@ struct b200_engine {
     DBUF(int32_t, ss_diff); DBUF(int32_t, ss_nplp); DBUF(uint32_t, ss_fail); DBUF(uint32_t, ss_extra); DBUF(b200_pileup1_t, ents);
     DBUF(int32_t, clip); DBUF(int64_t, next); DBUF(int32_t, cig_x); DBUF(int32_t, cig_y);
     DBUF(double, baq_f); DBUF(int32_t, baq_idx); DBUF(uint8_t, ref_codes); DBUF(uint16_t, ent); DBUF(uint16_t, ent2); DBUF(uint32_t, x_off); DBUF(char, x_dat); DBUF(int32_t, ov_pairs);
-    DBUF(float, gl_out); DBUF(int32_t, gl_n); DBUF(uint32_t, gl_flag); DBUF(uint32_t, cnt);   // cnt: planes of b200_mpileup_counts / _qsums / _psums bound for host memory
+    DBUF(float, gl_out); DBUF(int32_t, gl_n); DBUF(uint32_t, gl_flag); DBUF(uint32_t, cnt);   // cnt: planes of b200_mpileup_counts / _qsums / _psums / _ranksums bound for host memory
     // b200_mpileup_indels (mpileup_indel.cuh): per (column, file) event counts and offsets; per event the record (IndelEv),
     // symbol count, symbol offset, key, table slot, first-appearance flag and allele bytes, allele index and allele symbol
     // offset; 2 hash slots per event and their strand counts; the symbols of the events, then the table and its symbols
@@ -51,6 +51,8 @@ struct b200_engine {
     DBUF(uint64_t, ind_aseq); DBUF(int32_t, ind_tbl); DBUF(uint32_t, ind_tcnt); DBUF(char, ind_sym); DBUF(b200_indel_t, ind_tab); DBUF(char, ind_seq);
     DBUF(b200_indel_qsum_t, ind_qs);   // b200_indel_qsums: the rows of the table's quality sums
     DBUF(b200_indel_psum_t, ind_ps);   // b200_indel_psums: the rows of the table's read-position sums
+    // b200_mpileup_ranksums (mpileup_rank.cuh): per (file, column) the active flag and its exclusive scan, then the active list
+    DBUF(uint32_t, rk_act); DBUF(uint32_t, rk_off); DBUF(int32_t, rk_list);
     bool ind_ready = false; int64_t ind_n = 0; uint64_t ind_nseq = 0; uint32_t ind_nev = 0;   // the table of the staged batch: rows, symbol bytes, events
     void *d_acc = nullptr;
     unsigned long long *d_misc = nullptr;   // 64 words of small device results; slots MISC_* below, each zeroed by its writer's caller
@@ -79,7 +81,7 @@ struct b200_engine {
                        ref, dname, file_start, state, rlen, desc, endv, pmax, glo, ghi, status, out, bed_beg, bed_end, col_n,
                        col_off, col_state, tile_total, ovf_cnt, ovf_off, ovf_idx, ss_diff, ss_nplp, ss_fail, ss_extra, ents, clip, next, cig_x, cig_y, baq_f, baq_idx, ref_codes, ent, ent2, x_off, x_dat, ov_pairs, gl_out, gl_n, gl_flag, cnt,
                        ind_cnt, ind_off, ind_ev, ind_len, ind_soff, ind_key, ind_slot, ind_first, ind_bytes, ind_aidx, ind_aseq, ind_tbl, ind_tcnt,
-                       ind_sym, ind_tab, ind_seq, ind_qs, ind_ps, d_beta, d_fk, d_lhet, d_q2p, d_qthr };
+                       ind_sym, ind_tab, ind_seq, ind_qs, ind_ps, rk_act, rk_off, rk_list, d_beta, d_fk, d_lhet, d_q2p, d_qthr };
         for (void *p : ps) if (p) cudaFree(p);
     }
 };
@@ -94,6 +96,7 @@ enum : int {
     MISC_OVERLAP = 40,     // k_overlap: number of pairs to tweak; read by k_overlap_tweak
     MISC_QSUM_DEEP = 41,   // k_mp_qsums / k_ind_qsums: a column or allele too deep for 32-bit sums; read by their calls
     MISC_PSUM_OVF = 42,    // k_mp_psums / k_ind_psums: a sum of squared read positions past INT64_MAX; read by their calls
+    MISC_RANK_DEEP = 43,   // k_rank_counts: a column with more class entries than exact rank sums allow; read by b200_mpileup_ranksums
 };
 
 using plp::RawSoA;

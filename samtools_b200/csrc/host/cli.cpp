@@ -2,7 +2,8 @@
 // for the pileup hot path, driving the CUDA engine through its C ABI; `counts` prints the
 // per-column base and indel counts of mpileup's rows, `indels` the indel alleles of its
 // columns (both with --qsums: their base-quality and mapq sums, with --psums: their read-position
-// sums); `index` writes the BAI / CSI those commands read a region through.
+// sums; `counts --ranksums`: the rank-sum bias statistics of its columns); `index` writes the BAI /
+// CSI those commands read a region through.
 //
 // Option surfaces follow bam_plcmd.c:1096-1223 (mpileup), bam2depth.c:757-882
 // (depth) and coverage.c:343-424 (coverage), SURVEY.md Appendix B.  What stays
@@ -37,9 +38,9 @@
 
 using namespace b200;
 
-// The count, indel, quality-sum and position-sum outputs are optional parts of an engine build: the CLI links against any
-// implementation of the C ABI (the CUDA library, or a CPU debug build of the column code that may not provide them), and
-// `counts` / `indels` (or their --qsums / --psums) refuse to run on one without theirs.
+// The count, indel, quality-sum, position-sum and rank-sum outputs are optional parts of an engine build: the CLI links
+// against any implementation of the C ABI (the CUDA library, or a CPU debug build of the column code that may not provide
+// them), and `counts` / `indels` (or their --qsums / --psums / --ranksums) refuse to run on one without theirs.
 #pragma weak b200_mpileup_counts
 #pragma weak b200_mpileup_indels
 #pragma weak b200_fetch_indels
@@ -47,6 +48,7 @@ using namespace b200;
 #pragma weak b200_indel_qsums
 #pragma weak b200_mpileup_psums
 #pragma weak b200_indel_psums
+#pragma weak b200_mpileup_ranksums
 
 namespace {
 
@@ -142,6 +144,7 @@ struct WinWorker {
     std::vector<b200_indel_t> ind; std::string ind_seq;   // indel table of the window (indels)
     std::vector<uint32_t> qs; std::vector<b200_indel_qsum_t> ind_qs;   // quality sums of the window (--qsums)
     std::vector<int64_t> ps; std::vector<b200_indel_psum_t> ind_ps;    // position sums of the window (--psums)
+    std::vector<int64_t> rs;   // rank sums of the window (--ranksums)
     void rewind() { std::fill(cursor.begin(), cursor.end(), 0); }
     int fail(const char *tool) { rc = -1; err = std::string("samtools ") + tool + ": " + b200_last_error(eng.e); return -1; }
 };
@@ -325,6 +328,7 @@ struct MpOpts {
     bool indels = false;   // `indels`: the indel alleles of mpileup's columns (b200_mpileup_indels)
     bool qsums = false;    // --qsums: `counts` / `indels` add the quality sums (b200_mpileup_qsums / b200_indel_qsums)
     bool psums = false;    // --psums: `counts` / `indels` add the BP-5 sums (b200_mpileup_psums / b200_indel_psums), after any --qsums
+    bool ranksums = false; // --ranksums: `counts` adds the rank sums (b200_mpileup_ranksums), after any --qsums / --psums
     // host columns (bam_plcmd.c:727-855): record fields in the order of the MPLP_PRINT_* bits, then aux tags in the order given
     std::vector<std::string> xcols;      // "QNAME" "FLAG" "RNAME" "POS" "MAPQ" "RNEXT" "PNEXT" "RLEN" or a two-letter tag
     int n_xfields = 0;                   // how many of them are record fields (joined with ','; tags use x_sep)
@@ -550,6 +554,11 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn, const std::vector
                     w.ps.resize((size_t)nfn * B200_PSUM_PLANES * cap + 1);
                     if (b200_mpileup_psums(w.eng.e, o.min_baseQ, w.ps.data(), cap, &n) != 0) { w.fail("counts"); return; }
                 }
+                const int nr = o.ranksums ? B200_RANK_PLANES : 0;
+                if (o.ranksums) {
+                    w.rs.resize((size_t)nfn * B200_RANK_PLANES * cap + 1);
+                    if (b200_mpileup_ranksums(w.eng.e, o.min_baseQ, w.rs.data(), cap, &n) != 0) { w.fail("counts"); return; }
+                }
                 const int64_t n_all = std::min(we, h.lens[(size_t)tid]) - wb;
                 for (int64_t c = 0; c < n; ++c) {
                     bool any = false;
@@ -558,13 +567,14 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn, const std::vector
                     const int64_t p = wb + c;
                     if (o.bed && !o.bed->overlap(name, p, p + 1)) continue;
                     appendf(w, "%s\t%lld\t%c", name.c_str(), (long long)p + 1, (ref && p < (int64_t)ref->size()) ? (*ref)[(size_t)p] : 'N');
-                    const size_t need = w.need + (size_t)nfn * ((B200_COUNT_PLANES + nq) * 11 + np * 21) + 2;
+                    const size_t need = w.need + (size_t)nfn * ((B200_COUNT_PLANES + nq) * 11 + (np + nr) * 21) + 2;
                     if (w.out.size() < need) w.out.resize(std::max(2 * w.out.size(), need));
                     char *q = w.out.data() + w.need;
                     for (int f = 0; f < nfn; ++f) {
                         for (int k = 0; k < B200_COUNT_PLANES; ++k) { *q++ = '\t'; q = std::to_chars(q, w.out.data() + w.out.size(), w.cnt[((size_t)f * B200_COUNT_PLANES + (size_t)k) * plane + (size_t)c]).ptr; }
                         for (int k = 0; k < nq; ++k) { *q++ = '\t'; q = std::to_chars(q, w.out.data() + w.out.size(), w.qs[((size_t)f * B200_QSUM_PLANES + (size_t)k) * plane + (size_t)c]).ptr; }
                         for (int k = 0; k < np; ++k) { *q++ = '\t'; q = std::to_chars(q, w.out.data() + w.out.size(), w.ps[((size_t)f * B200_PSUM_PLANES + (size_t)k) * plane + (size_t)c]).ptr; }
+                        for (int k = 0; k < nr; ++k) { *q++ = '\t'; q = std::to_chars(q, w.out.data() + w.out.size(), w.rs[((size_t)f * B200_RANK_PLANES + (size_t)k) * plane + (size_t)c]).ptr; }
                     }
                     *q++ = '\n';
                     w.need = (size_t)(q - w.out.data());
@@ -669,7 +679,8 @@ int main_mpileup(int argc, char **argv, MpCmd cmd)
         {"output-mods", 0, 0, 'M'}, {"output-BP", 0, 0, 'O'}, {"output-bp", 0, 0, 'O'}, {"output-BP-5", 0, 0, 14}, {"output-bp-5", 0, 0, 14},
         {"output-MQ", 0, 0, 's'}, {"output-mq", 0, 0, 's'}, {"customized-index", 0, 0, 'X'}, {"reverse-del", 0, 0, 6},
         {"output-extra", 1, 0, 7}, {"output-sep", 1, 0, 8}, {"output-empty", 1, 0, 9}, {"no-output-ins", 0, 0, 10},
-        {"no-output-ins-mods", 0, 0, 11}, {"no-output-del", 0, 0, 12}, {"no-output-ends", 0, 0, 13}, {"qsums", 0, 0, 15}, {"psums", 0, 0, 16}, {0, 0, 0, 0} };
+        {"no-output-ins-mods", 0, 0, 11}, {"no-output-del", 0, 0, 12}, {"no-output-ends", 0, 0, 13}, {"qsums", 0, 0, 15}, {"psums", 0, 0, 16},
+        {"ranksums", 0, 0, 17}, {0, 0, 0, 0} };
     int c;
     optind = 1;
     while ((c = getopt_long(argc, argv, "Af:r:l:q:Q:RC:Bd:b:o:EG:6OsxXaM", lo, nullptr)) >= 0) {
@@ -678,6 +689,7 @@ int main_mpileup(int argc, char **argv, MpCmd cmd)
             fprintf(stderr, "b200samtools %s: %s is an option of the pileup text\n\n"
                             "Usage: b200samtools %s [-f ref.fa] [-r reg] [-l bed] [-b list] [-X] [-q INT] [-Q INT] [-B] [-E] [-C INT] [-d INT]\n"
                             "                           [-x] [-A] [-6] [-G file] [-R] [--rf FLAGS] [--ff FLAGS] [-a[a]] [-o out] [--qsums] [--psums]\n"
+                            "                           [--ranksums (counts)]\n"
                             "                           in1.bam [in2.bam ...]\n",
                     tool, c < 32 ? argv[optind - 1] : opt, tool);
             return 1;
@@ -721,6 +733,9 @@ int main_mpileup(int argc, char **argv, MpCmd cmd)
         case 16:
             if (!o.counts && !o.indels) { fprintf(stderr, "b200samtools mpileup: --psums is an option of `counts` and `indels`\n"); return 1; }
             o.psums = true; break;
+        case 17:
+            if (!o.counts) { fprintf(stderr, "b200samtools %s: --ranksums is an option of `counts`\n", o.indels ? "indels" : "mpileup"); return 1; }
+            o.ranksums = true; break;
         case 'f': o.fa = Fasta::load(optarg); if (!o.fa) { fprintf(stderr, "[E::fai_load] failed to open %s\n", optarg); return 1; } o.fa_fn = optarg; break;
         case 'd': o.max_depth = atoi(optarg); break;
         case 'r': o.reg = optarg; break;
@@ -751,6 +766,7 @@ int main_mpileup(int argc, char **argv, MpCmd cmd)
     if (o.indels && (!b200_mpileup_indels || !b200_fetch_indels)) { fprintf(stderr, "b200samtools indels: this engine build has no indel output\n"); return 1; }
     if (o.qsums && (o.counts ? !b200_mpileup_qsums : !b200_indel_qsums)) { fprintf(stderr, "b200samtools %s: this engine build has no quality sums\n", tool); return 1; }
     if (o.psums && (o.counts ? !b200_mpileup_psums : !b200_indel_psums)) { fprintf(stderr, "b200samtools %s: this engine build has no position sums\n", tool); return 1; }
+    if (o.ranksums && !b200_mpileup_ranksums) { fprintf(stderr, "b200samtools counts: this engine build has no rank sums\n"); return 1; }
     if (!o.realn && o.redo_baq) { fprintf(stderr, "Error: The -B option cannot be combined with -E\n"); return 1; }
     if (use_orphan) o.no_orphan = false;
     {   // record fields print in the order of the MPLP_PRINT_* bits (bam_plcmd.c:185-196,728-795), tags after them in the order given

@@ -483,6 +483,50 @@ PLP_HD EntPs mp_entry_ps(const ReadDesc &d, const Ent &e)
 // holds for a lane-private cell and for the old value an atomicAdd returns alike.
 PLP_HD bool ps_sq_over(uint64_t old, uint64_t x) { return old + x > (uint64_t)INT64_MAX; }
 
+// ---- per-column rank sums of the entries (mpileup_rank.cuh): Mann-Whitney U of BQ, MQ and BP-5, ref against alt ---------
+// A class entry is an entry that passes -Q and whose kind (mp_entry_channel & 15) is A, C, G or T: of the ref class where
+// the text prints it as '.' / ',' (mp_entry_base == 0), of the alt class otherwise (every non-reference base pooled).  Its
+// values are BQ and MQ as mp_entry_qs gives them (0..93) and its BP-5 (qpos5_of; >= 1 for a class entry, whose base lies
+// inside SEQ) capped at RS_POS_CAP: a BP-5 above the cap ranks as the cap, which keeps the position histogram at a fixed
+// size.  Planes per file: n_ref, n_alt, then U2 and T of BQ, of MQ and of the BP-5 (RS_U2 + 2 * var, RS_U2 + 2 * var + 1):
+//   U2 = sum over (alt a, ref r) of 2 [a > r] + [a == r]   (2 U of the alt sample, an integer)
+//   T  = sum over values v of t_v^3 - t_v                   (t_v: the class entries, ref and alt, of value v)
+// both 0 unless both classes have entries.  T <= n^3 - n for n class entries: exact in int64 while n <= RS_MAX_DEPTH.
+enum { RS_NREF = 0, RS_NALT = 1, RS_U2 = 2, RS_PLANES = B200_RANK_PLANES };
+enum { RS_NONE = 0, RS_REF = 1, RS_ALT = 2 };
+// one histogram of a class: RS_QBINS bins of BQ, RS_QBINS of MQ, RS_POS_CAP of BP-5 (var v starts at bin v * RS_QBINS)
+constexpr int RS_QBINS = 94, RS_POS_CAP = 1024, RS_BINS = 2 * RS_QBINS + RS_POS_CAP;
+constexpr uint32_t RS_MAX_DEPTH = 2097151;   // 2^21 - 1: n^3 - n < 2^63 (with a margin of one: 2^21 + 1 would wrap)
+PLP_HD int rs_nbins(int var) { return var < 2 ? RS_QBINS : RS_POS_CAP; }
+struct EntRank { int cls; int bin[3]; };
+// an entry that passes -Q (q: ent_qual) of read d at column c: its class (RS_NONE / RS_REF / RS_ALT) and its BQ, MQ and
+// BP-5 bins in [0, RS_BINS), each inside its value's range whatever the descriptor holds
+PLP_HD EntRank mp_entry_rank(const View &v, const ReadDesc &d, const Ent &e, int32_t c, int q)
+{
+    EntRank r;
+    const int kind = mp_entry_channel(v, d, v.cigar + d.cig_off, e, c) & 15;
+    r.cls = kind > CNT_T ? RS_NONE : mp_entry_base(v, d, e, c) == 0 ? RS_REF : RS_ALT;
+    const EntQs x = mp_entry_qs(q, d);
+    const int32_t p = qpos5_of(d, e);
+    r.bin[0] = (int)x.bq;
+    r.bin[1] = RS_QBINS + (int)x.mq;
+    r.bin[2] = 2 * RS_QBINS + (p < 1 ? 0 : p > RS_POS_CAP ? RS_POS_CAP - 1 : p - 1);
+    return r;
+}
+// U2 and T (above) of one value's histograms ref[0, nbins) and alt[0, nbins), added to u2 and t.  below: the ref entries of
+// lower value than bin 0 (a warp splits the bins into runs, each lane starting from the ref entries below its run).
+PLP_HD void rank_from_hist(const uint32_t *ref, const uint32_t *alt, int nbins, uint64_t &u2, uint64_t &t, uint64_t below = 0)
+{
+    for (int b = 0; b < nbins; ++b) {
+        const uint64_t r = ref[b], a = alt[b], n = r + a;
+        u2 += a * (2 * below + r);
+        t += n * n * n - n;
+        below += r;
+    }
+}
+// true where a column's n class entries are too many for exact planes (the call then fails instead of wrapping)
+PLP_HD bool rank_depth_over(uint64_t n) { return n > RS_MAX_DEPTH; }
+
 // ---- indel alleles of the entries (mpileup_indel.cuh): the distinct "+n..." / "-n" tokens of one (column, file) ---------
 // An allele is its signed length (>= 0: an insertion of that many symbols, forward-strand form from ins_symbols; < 0: a
 // deletion of -len reference bases, which name it by length alone) and, for an insertion, the symbol bytes.  Two tokens are

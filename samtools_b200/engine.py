@@ -22,12 +22,13 @@ EXPORTS = ['b200_engine_create', 'b200_engine_destroy', 'b200_last_error', 'b200
            'b200_launch_count', 'b200_last_mpileup_parts_ms', 'b200_gl_rng_draws', 'b200_last_baq_ms',
            'b200_errmod_cal', 'b200_glfgen', 'b200_cap_mapq', 'b200_mpileup_text_bound', 'b200_depth_text_bound', 'b200_bedcov',
            'b200_mpileup_counts', 'b200_mpileup_indels', 'b200_fetch_indels', 'b200_mpileup_qsums', 'b200_indel_qsums',
-           'b200_mpileup_psums', 'b200_indel_psums']
+           'b200_mpileup_psums', 'b200_indel_psums', 'b200_mpileup_ranksums']
 COUNT_PLANES = 19   # b200_mpileup_counts: per file A C G T N del skip +ins -del, forward then reverse strand, then n_plp
 QSUM_PLANES = 42    # b200_mpileup_qsums: per file BQ sums, MQ sums, MQ0 counts, each of A C G T N del skip, forward then reverse
 # b200_indel_qsum_t, one row of b200_indel_qsums beside the row of b200_mpileup_indels
 INDEL_QSUM_FIELDS = ('bq_fwd', 'bq_rev', 'mq_fwd', 'mq_rev', 'mq0_fwd', 'mq0_rev')
 PSUM_PLANES = 28    # b200_mpileup_psums: per file BP-5 sums, sums of BP-5 squared, each of A C G T N del skip, forward then reverse
+RANK_PLANES = 8     # b200_mpileup_ranksums: per file n_ref, n_alt, then U2 and T of BQ, of MQ and of BP-5 (capped at 1024)
 
 
 class IndelPsum(C.Structure):
@@ -114,6 +115,7 @@ def load_library():
         lib.b200_indel_qsums.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_mpileup_psums.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64)]
         lib.b200_indel_psums.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
+        lib.b200_mpileup_ranksums.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_size_t, C.POINTER(C.c_int64)]
         lib.b200_fetch_qual.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_fetch_mapq_keep.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t]
         lib.b200_pileup_entries.argtypes = [C.c_void_p, C.c_int32, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]
@@ -150,6 +152,27 @@ def default_stage_conf(mode=MODE_MPILEUP, **kw):
             raise AttributeError(k)
         setattr(c, k, v)
     return c
+
+
+def ranksum_z(planes):
+    """z-scores of the rank-sum planes of Engine.mpileup_ranksums (numpy or torch int64, [..., 8, n]): float64 [..., 3, n]
+    for BQ, MQ and the BP-5, of the same kind and on the same device.  With n1 = n_ref, n2 = n_alt, N = n1 + n2 and per
+    value U = U2 / 2, mu = n1 n2 / 2 and sigma^2 = n1 n2 / 12 ((N + 1) - T / (N (N - 1))) (the tie-corrected normal
+    approximation, no continuity correction), z = (U - mu) / sigma: positive where the non-reference bases have the larger
+    values.  NaN where a class is empty or sigma = 0 (every entry of the column has the same value)."""
+    import sys
+    torch = sys.modules.get('torch')
+    is_t = torch is not None and isinstance(planes, torch.Tensor)
+    f64 = (lambda a: a.to(torch.float64)) if is_t else (lambda a: np.asarray(a).astype(np.float64))
+    n1, n2 = planes[..., 0:1, :], planes[..., 1:2, :]
+    u2, t = planes[..., 2::2, :], planes[..., 3::2, :]
+    n = n1 + n2
+    num = (n + 1) * n * (n - 1) - t                # 12 N (N - 1) sigma^2 / (n1 n2), exact in int64
+    ok = (n1 > 0) & (n2 > 0) & (num > 0)
+    with np.errstate(divide='ignore', invalid='ignore'):
+        var = f64(n1) * f64(n2) * f64(num) / (12.0 * f64(n) * f64(n - 1))
+        z = (f64(u2) / 2 - f64(n1) * f64(n2) / 2) / (var.sqrt() if is_t else np.sqrt(var))
+    return z.masked_fill(~ok, float('nan')) if is_t else np.where(ok, z, np.nan)
 
 
 class Engine:
@@ -297,6 +320,13 @@ class Engine:
         BP-5 sums and sums of BP-5 squared (plane s * 14 + strand * 7 + kind), or, given `out`, a contiguous torch.int64 CUDA
         tensor of that shape on the handle's device, filled in place on the device (and returned)."""
         return self._planes('b200_mpileup_psums', PSUM_PLANES, min_baseQ, out, np.int64, 'int64')
+
+    def mpileup_ranksums(self, min_baseQ=13, out=None):
+        """Per-column rank-sum bias statistics of the staged window (b200_mpileup_ranksums): a numpy int64 [n_files, 8, n]
+        array of n_ref, n_alt and, for BQ, MQ and the BP-5 (capped at 1024) in turn, U2 (twice the Mann-Whitney U of the
+        non-reference bases) and the tie term T; or, given `out`, a contiguous torch.int64 CUDA tensor of that shape on the
+        handle's device, filled in place on the device (and returned).  ranksum_z turns the planes into z-scores."""
+        return self._planes('b200_mpileup_ranksums', RANK_PLANES, min_baseQ, out, np.int64, 'int64')
 
     def mpileup_indels(self, min_baseQ=13, device=False):
         """Per-column indel alleles of the staged window (b200_mpileup_indels): (rows, symbols).  By default a numpy structured
