@@ -387,6 +387,17 @@ static int launch_scan(b200_engine *e, const In *in, Out *out, int64_t n)
     k_scan<Op, IPT, INCL><<<nb, SCAN_T, 0, e->stream>>>(in, out, (int32_t)n, st, ticket); e->launches++;
     return 0;
 }
+// b200_mpileup_indels, b200_mpileup_ranksums and b200_glf keep one entry per (column, file) pair of the window in tables
+// they index and scan in 32 bits.  They refuse a window past this many pairs before allocating anything; the CLI's windows
+// (2^24 pairs) stay far below it.
+constexpr int64_t MAX_COL_FILE_PAIRS = INT32_MAX - SCAN_T * 4;
+static bool col_file_pairs_over(b200_engine *e, int64_t ncols)
+{
+    if (ncols * e->n_files <= MAX_COL_FILE_PAIRS) return false;
+    snprintf(e->err, sizeof e->err, "window too large: %lld columns x %d files exceed the limit of %lld (column, file) pairs",
+             (long long)ncols, e->n_files, (long long)MAX_COL_FILE_PAIRS);
+    return true;
+}
 
 #include "overlap.cuh"
 #include "baq.cuh"
@@ -909,10 +920,11 @@ extern "C" int b200_mpileup_text(b200_engine_t *e, const b200_mpileup_conf_t *c,
 // The planes of b200_mpileup_counts, b200_mpileup_qsums, b200_mpileup_psums and b200_mpileup_ranksums: checks,
 // destination, the kernels (launch(blocks, view, n_groups, dst), nonzero on an error: k_mp_counts, k_mp_qsums, k_mp_psums,
 // or the two phases of mpileup_rank.cuh), the copy to host memory.  T: the cell type.  flag: the d_misc slot where a kernel
-// flags a value it could not keep exact, or nullptr; the call then fails with flag_msg.
+// flags a value it could not keep exact, or nullptr; the call then fails with flag_msg.  pair_tables: the launch keeps
+// tables of (column, file) pairs (col_file_pairs_over).
 template <class T, class Launch>
 static int col_planes(b200_engine *e, const char *what, const char *buf, int planes, T *out, size_t cap_cols, int64_t *n_cols,
-                      unsigned long long *flag, const char *flag_msg, Launch launch)
+                      unsigned long long *flag, const char *flag_msg, bool pair_tables, Launch launch)
 {
     if (!e || !e->staged) { if (e) snprintf(e->err, sizeof e->err, "no staged batch"); return -1; }
     if (e->sconf.mode != B200_MODE_MPILEUP) { snprintf(e->err, sizeof e->err, "mpileup %s need a batch staged in B200_MODE_MPILEUP", what); return -1; }
@@ -922,6 +934,7 @@ static int col_planes(b200_engine *e, const char *what, const char *buf, int pla
     *n_cols = n; e->last_kernel_ms = 0;
     if (out && cap_cols < (size_t)n) { snprintf(e->err, sizeof e->err, "%s buffer too small: need %lld columns", buf, (long long)n); return -2; }
     if (n == 0) return 0;
+    if (pair_tables && col_file_pairs_over(e, n)) return -1;
     // the kernel writes straight into a caller's device buffer; host memory gets the planes through the handle's buffer
     T *dst = nullptr;
     if (out) {
@@ -952,7 +965,7 @@ static int col_planes(b200_engine *e, const char *what, const char *buf, int pla
 
 extern "C" int b200_mpileup_counts(b200_engine_t *e, int32_t min_baseQ, uint32_t *out, size_t cap_cols, int64_t *n_cols)
 {
-    return col_planes(e, "counts", "count", CNT_PLANES, out, cap_cols, n_cols, nullptr, nullptr, [&](int blocks, const View &v, int32_t n_groups, uint32_t *dst) {
+    return col_planes(e, "counts", "count", CNT_PLANES, out, cap_cols, n_cols, nullptr, nullptr, false, [&](int blocks, const View &v, int32_t n_groups, uint32_t *dst) {
         k_mp_counts<<<blocks, CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, dst);
         return 0;
     });
@@ -963,7 +976,7 @@ extern "C" int b200_mpileup_qsums(b200_engine_t *e, int32_t min_baseQ, uint32_t 
     unsigned long long *deep = e ? e->d_misc + MISC_QSUM_DEEP : nullptr;
     char msg[96];
     snprintf(msg, sizeof msg, "a column has more than %u reads: its quality sums would not fit in 32 bits", QS_MAX_DEPTH);
-    return col_planes(e, "quality sums", "quality sum", QS_PLANES, out, cap_cols, n_cols, deep, msg, [&](int blocks, const View &v, int32_t n_groups, uint32_t *dst) {
+    return col_planes(e, "quality sums", "quality sum", QS_PLANES, out, cap_cols, n_cols, deep, msg, false, [&](int blocks, const View &v, int32_t n_groups, uint32_t *dst) {
         k_mp_qsums<<<blocks, CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, dst, deep);
         return 0;
     });
@@ -973,7 +986,7 @@ extern "C" int b200_mpileup_psums(b200_engine_t *e, int32_t min_baseQ, int64_t *
 {
     unsigned long long *ovf = e ? e->d_misc + MISC_PSUM_OVF : nullptr;
     return col_planes(e, "position sums", "position sum", PS_PLANES, out, cap_cols, n_cols, ovf,
-                      "a column's sum of squared read positions would exceed 2^63 - 1", [&](int blocks, const View &v, int32_t n_groups, int64_t *dst) {
+                      "a column's sum of squared read positions would exceed 2^63 - 1", false, [&](int blocks, const View &v, int32_t n_groups, int64_t *dst) {
         k_mp_psums<<<blocks, CNT_WARPS * 32, 0, e->stream>>>(v, min_baseQ, n_groups, dst, ovf);
         return 0;
     });
@@ -984,7 +997,7 @@ extern "C" int b200_mpileup_ranksums(b200_engine_t *e, int32_t min_baseQ, int64_
     unsigned long long *deep = e ? e->d_misc + MISC_RANK_DEEP : nullptr;
     char msg[128];
     snprintf(msg, sizeof msg, "a column has more than %u reference and non-reference bases: its rank sums would not fit in 64 bits", RS_MAX_DEPTH);
-    return col_planes(e, "rank sums", "rank sum", RS_PLANES, out, cap_cols, n_cols, deep, msg, [&](int blocks, const View &v, int32_t n_groups, int64_t *dst) {
+    return col_planes(e, "rank sums", "rank sum", RS_PLANES, out, cap_cols, n_cols, deep, msg, true, [&](int blocks, const View &v, int32_t n_groups, int64_t *dst) {
         // the list of active (file, column) pairs is sized by all of them; phase 2 reads its length from HBM
         const int64_t pairs = (int64_t)e->n_files * v.ncols;
         ENSURE(rk_act, (size_t)pairs); ENSURE(rk_off, (size_t)pairs + 1); ENSURE(rk_list, (size_t)pairs);
@@ -1019,7 +1032,8 @@ extern "C" int b200_mpileup_indels(b200_engine_t *e, int32_t min_baseQ, int64_t 
     // P / D op of its read, and its symbols are the lengths of the I / P ops after the entry
     const uint64_t ops = e->sum_indel_text - 3ull * (uint64_t)e->acc_n_kept;
     const uint64_t cap64 = ops / 12 + 1, sym_cap = ops + 1;
-    if (segs + 2 > INT32_MAX || cap64 > (uint64_t)INT32_MAX / 2) { snprintf(e->err, sizeof e->err, "window too large for the indel table"); return -1; }
+    if (col_file_pairs_over(e, n)) return -1;
+    if (cap64 > (uint64_t)INT32_MAX / 2) { snprintf(e->err, sizeof e->err, "window too large for the indel table"); return -1; }
     const uint32_t cap = (uint32_t)cap64;
     if (n == 0) { e->ind_ready = true; return 0; }
     ENSURE(ind_cnt, (size_t)segs + 1); ENSURE(ind_off, (size_t)segs + 2);

@@ -232,9 +232,10 @@ extern "C" int b200_glf(b200_engine_t *e, int32_t min_baseQ, int64_t *n_cols, in
 {
     if (!e || !e->staged) { if (e) snprintf(e->err, sizeof e->err, "no staged batch"); return -1; }
     CK(cudaSetDevice(e->device));
-    if (errmod_tables(e, 1. - 0.83)) return -1;
     View v; fill_view(e, v, nullptr, nullptr, 0, 0, 0);
     *n_cols = 0;
+    if (col_file_pairs_over(e, v.ncols)) return -1;
+    if (errmod_tables(e, 1. - 0.83)) return -1;
     const int64_t tot = (int64_t)v.ncols * v.n_files;
     if (tot == 0) return 0;
     ENSURE(col_n, (size_t)tot + 1); ENSURE(col_off, (size_t)tot + 2); ENSURE(gl_n, (size_t)tot + 1);

@@ -290,11 +290,14 @@ bool column_range(const std::vector<FileData> &fd, int tid, int64_t tid_len, int
     if (!all) { lo = std::max(rb, first); hi = std::min(re, last); } else hi = std::max(hi, std::min(re, last));
     return lo < hi;
 }
-// [lo,hi) cut into windows of window_cols() columns; an empty range is still one (empty) window
-Windows column_windows(int64_t lo, int64_t hi)
+// [lo,hi) of a run over n_files files cut into windows of window_cols() columns, and of at most 2^24 (column, file) pairs:
+// a window's buffers grow with its columns times the files (the text bounds, the count and sum planes, the indel, rank-sum
+// and GL tables), so a cohort's windows hold what one file's 2^24 columns hold.  An empty range is still one (empty) window.
+Windows column_windows(int64_t lo, int64_t hi, int n_files)
 {
+    const int64_t w = std::min(window_cols(), std::max<int64_t>(1, (1LL << 24) / std::max(n_files, 1)));
     Windows wins;
-    for (int64_t wb = lo; wb < hi || wb == lo; wb += window_cols()) wins.emplace_back(wb, std::max(std::min(wb + window_cols(), hi), wb));
+    for (int64_t wb = lo; wb < hi || wb == lo; wb += w) wins.emplace_back(wb, std::max(std::min(wb + w, hi), wb));
     return wins;
 }
 // Stages window [wb,we) of contig tid on worker w: add(i) packs into w.pb the records file i contributes (w.cursor[i] and
@@ -486,7 +489,7 @@ int run_mpileup(MpOpts &o, const std::vector<std::string> &fn, const std::vector
             if (with_reads && tid < (int)fd[(size_t)i].by_tid.size())
                 for (Record &r : fd[(size_t)i].by_tid[(size_t)tid]) hbits[(size_t)i].push_back(mp_host_bits(o, h, r, ref != nullptr));
         }
-        const Windows wins = column_windows(lo, hi);
+        const Windows wins = column_windows(lo, hi, nfn);
         // a window that continues an earlier one also takes the records ending at its start (the -d rule's closed intervals)
         auto stage = [&](WinWorker &w, int64_t wb, int64_t we, b200_stage_stats_t &st) {
             if (!o.xcols.empty()) staged.clear();
@@ -894,7 +897,7 @@ int main_depth(int argc, char **argv)
         if (bed) { bed->merged(name, bb, be); dc.bed_beg = bb.data(); dc.bed_end = be.data(); dc.n_bed = (int)bb.size(); dc.bed_active = 1; }
         int64_t lo = 0, hi = 0;
         if (!column_range(fd, tid, h.lens[(size_t)tid], beg0, end0, all_pos, with_reads, lo, hi)) return 0;
-        const Windows wins = column_windows(lo, hi);
+        const Windows wins = column_windows(lo, hi, nfn);
         auto stage = [&](WinWorker &w, int64_t wb, int64_t we, b200_stage_stats_t &st) {
             return stage_window(w, h, tid, nullptr, sc, wb, we, nullptr, "depth", st, [&](int i) {
                 if (!with_reads || tid >= (int)fd[(size_t)i].by_tid.size()) return;
@@ -1036,7 +1039,7 @@ int main_coverage(int argc, char **argv)
         // the first / last window also take the records that lie before / beyond the region.
         // A window that continues an earlier one also stages the records ending right at its start (the closed intervals
         // of the -d rule; they cover none of its columns), and where the rule may fire the windows hand their verdicts on.
-        const Windows wins = column_windows(rw.beg, rw.end);
+        const Windows wins = column_windows(rw.beg, rw.end, nfn);
         md.reset(fd, tid, wins.size() > 1 && max_stacked_records(fd, tid) > (int64_t)sc.max_depth);
         const int rc = run_window_rounds(workers, wins, 1, fp, [&](WinWorker &w, int64_t wb, int64_t we) {
             const bool first_w = wb == rw.beg, last_w = we >= rw.end;
