@@ -105,6 +105,21 @@ __global__ void k_build_desc(RawSoA r, b200_stage_conf_t cf, const uint8_t *stat
         stage_build_desc(r, cf, i, state, rlen, desc, endv, &loc, win_base, cig_x, cig_y);
     merge_acc(loc, acc);
 }
+// The three kernels above in one pass, for a stage without BAQ (which has to run between stage_prep1 and stage_prep2):
+// each function reads and writes nothing but read i (and the raw pos[i - 1]), so one thread can run them in order.  One
+// accumulator takes both stage_prep1's coverage counters and stage_build_desc's sums; its one merge gives what the two
+// merges of k_prep1 and k_build_desc give.
+__global__ void __launch_bounds__(256, 4) k_prep_desc(RawSoA r, b200_stage_conf_t cf, uint8_t *state, int32_t *rlen, ReadDesc *desc, int32_t *endv, StageAcc *acc,
+                            int64_t win_base, int32_t *cig_x, int32_t *cig_y)
+{
+    StageAcc loc; memset(&loc, 0, sizeof loc); loc.max_rend = INT32_MIN;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < r.n; i += (int64_t)gridDim.x * blockDim.x) {
+        stage_prep1(r, cf, i, state, rlen, &loc);
+        stage_prep2(r, cf, i, state);
+        stage_build_desc(r, cf, i, state, rlen, desc, endv, &loc, win_base, cig_x, cig_y);
+    }
+    merge_acc(loc, acc);
+}
 
 // per 32-column group: the [lo,hi) slice of each file's reads that can cover it (plp_stage.h group_slice)
 __global__ void k_ranges(const ReadDesc *desc, const int32_t *pmax, const int64_t *file_start, int n_files,
@@ -562,6 +577,7 @@ extern "C" int b200_stage(b200_engine_t *e, const b200_batch_t *b, const b200_st
     if (n >= (1LL << 31)) { snprintf(e->err, sizeof e->err, "batch too large (%lld reads)", (long long)n); return -1; }
     if (b->qual_bytes >= (1ULL << 32) || b->n_cigar_total >= (1ULL << 32)) { snprintf(e->err, sizeof e->err, "batch payload exceeds 4 GiB: split the window"); return -1; }
     CK(cudaEventRecord(e->ev0, e->stream));
+    e->qual_state = QUAL_DIRTY;   // a new batch: qual holds nothing of its qual0 yet
     e->n = n; e->n_files = b->n_files; e->tid = b->tid; e->tid_len = b->tid_len;
     e->name = b->tid_name ? b->tid_name : "";
     e->sconf = *cf;
@@ -611,10 +627,8 @@ static int stage_device(b200_engine *e, b200_stage_stats_t *stats)
     e->ind_ready = false;   // the indel table belongs to the batch it was computed on
     const int64_t n = e->n;
     const b200_stage_conf_t *cf = &e->sconf;
-    if (e->keep_raw && n > 0) {
-        CK(cudaMemcpyAsync(e->qual, e->qual0, e->qual_bytes, cudaMemcpyDeviceToDevice, e->stream));
-        CK(cudaMemcpyAsync(e->mapq, e->mapq0, (size_t)n, cudaMemcpyDeviceToDevice, e->stream));
-    }
+    const QualState qual_was = e->qual_state;
+    e->qual_state = QUAL_DIRTY;   // until this stage completes
     ENSURE(state, (size_t)n + 1); ENSURE(rlen, (size_t)n + 1); ENSURE(desc, (size_t)n + 1);
     ENSURE(endv, (size_t)n + 1); ENSURE(pmax, (size_t)n + 1);
     ENSURE(cig_x, e->n_cigar_total + 1); ENSURE(cig_y, e->n_cigar_total + 1);
@@ -630,23 +644,30 @@ static int stage_device(b200_engine *e, b200_stage_stats_t *stats)
     r.cigar = e->cigar; r.seq4 = e->seq4; r.qual = e->qual;
     r.ref = e->has_ref ? e->ref : nullptr; r.ref_beg = e->ref_beg; r.ref_n = e->ref_n; r.ref_len = e->ref_len;
     r.n = n; r.tid = e->tid;
+    if (e->keep_raw && n > 0) {   // back to the pristine qualities (undoing only what the last stage edited) and mapq
+        if (qual_was == QUAL_DIRTY) CK(cudaMemcpyAsync(e->qual, e->qual0, e->qual_bytes, cudaMemcpyDeviceToDevice, e->stream));
+        else if (qual_was == QUAL_PAIRS && launch_qual_restore(e, r)) return -1;
+        CK(cudaMemcpyAsync(e->mapq, e->mapq0, (size_t)n, cudaMemcpyDeviceToDevice, e->stream));
+    }
     StageAcc *acc = (StageAcc *)e->d_acc;
     if (e->has_ref && e->ref_n > 0) {   // reference bases -> codes, once per staged batch (BAQ: 0..4, pileup_seq: nt16)
         ENSURE(ref_codes, (size_t)e->ref_n + 1);
         k_ref_codes<<<nblk(e->ref_n, 256), 256, 0, e->stream>>>(e->ref, e->ref_n, e->ref_codes); e->launches++;
     }
+    e->baq_ran = false;
     if (n > 0) {
         const int gs = (int)std::min<int64_t>(nblk(n, 256), (int64_t)e->n_sm * 16);   // grid-stride: one set of accumulator atomics per block
-        k_prep1<<<gs, 256, 0, e->stream>>>(r, *cf, e->state, e->rlen, acc); e->launches++;
-        e->baq_ran = false;
         if (cf->mode == B200_MODE_MPILEUP && cf->baq && e->has_ref) {
+            k_prep1<<<gs, 256, 0, e->stream>>>(r, *cf, e->state, e->rlen, acc); e->launches++;
             CK(cudaEventRecord(e->evB0, e->stream));
             if (launch_baq(e, r, *cf)) return -1;
             CK(cudaEventRecord(e->evB1, e->stream));
             e->baq_ran = true;
+            k_prep2<<<nblk(n, 256), 256, 0, e->stream>>>(r, *cf, e->state); e->launches++;
+            k_build_desc<<<gs, 256, 0, e->stream>>>(r, *cf, e->state, e->rlen, e->desc, e->endv, acc, e->win_base, e->cig_x, e->cig_y); e->launches++;
+        } else {
+            k_prep_desc<<<gs, 256, 0, e->stream>>>(r, *cf, e->state, e->rlen, e->desc, e->endv, acc, e->win_base, e->cig_x, e->cig_y); e->launches++;
         }
-        k_prep2<<<nblk(n, 256), 256, 0, e->stream>>>(r, *cf, e->state); e->launches++;
-        k_build_desc<<<gs, 256, 0, e->stream>>>(r, *cf, e->state, e->rlen, e->desc, e->endv, acc, e->win_base, e->cig_x, e->cig_y); e->launches++;
     }
     CK(cudaGetLastError());
     // ---- statistics back (also the sync point that validates the batch)
@@ -666,6 +687,7 @@ static int stage_device(b200_engine *e, b200_stage_stats_t *stats)
     ENSURE(glo, (size_t)e->n_groups * e->n_files + 1); ENSURE(ghi, (size_t)e->n_groups * e->n_files + 1);
     e->maxdrop_applied = false;
     int max_range = 0;
+    bool tweaked = false;
     if (n > 0) {
         if (build_ranges(e, &max_range)) return -1;
         bool may_fire = max_depth_may_fire(*cf, max_range);
@@ -683,7 +705,7 @@ static int stage_device(b200_engine *e, b200_stage_stats_t *stats)
                 if (build_ranges(e, &max_range)) return -1;
             }
         }
-        if (cf->mode == B200_MODE_MPILEUP && cf->overlaps && e->has_prev) { if (launch_overlap(e, r)) return -1; }
+        if (cf->mode == B200_MODE_MPILEUP && cf->overlaps && e->has_prev) { if (launch_overlap(e, r)) return -1; tweaked = true; }
         if (e->has_host_clip) {
             e->has_clip = true;
         } else if (cf->mode == B200_MODE_DEPTH && cf->d_remove_overlaps && e->has_prev) { if (launch_depth_clip(e, r)) return -1; }
@@ -701,6 +723,7 @@ static int stage_device(b200_engine *e, b200_stage_stats_t *stats)
     cudaEventElapsedTime(&ms, e->evA, e->ev1); e->last_stage_device_ms = ms;
     e->last_baq_ms = 0;
     if (e->baq_ran) { cudaEventElapsedTime(&ms, e->evB0, e->evB1); e->last_baq_ms = ms; }
+    if (e->keep_raw && n > 0) e->qual_state = (e->baq_ran || cf->illumina13) ? QUAL_DIRTY : tweaked ? QUAL_PAIRS : QUAL_PRISTINE;
     e->staged = true;
     if (stats) {
         stats->n_kept = (int64_t)ha.n_kept; stats->n_kept_in_window = (int64_t)ha.n_kept_in_window;

@@ -9,6 +9,21 @@
 
 #define DBUF(type, name) type *name = nullptr; size_t cap_##name = 0
 
+// What b200_restage has to undo in the staged qualities (e->qual) before it repeats the read stage: everything (a full
+// copy from qual0), the mates of the pairs the last overlap tweak listed (k_qual_restore), or nothing.  The device
+// writers of e->qual, each of which must be accounted for here:
+//   stage_prep1 (plp_stage.h)                -6 (cf.illumina13)                       -> QUAL_DIRTY
+//   k_baq / k_baq_reg (baq.cuh, baq_reg.h)   BAQ                                      -> QUAL_DIRTY
+//   k_overlap_tweak (overlap.cuh)            mates of the pairs in ov_pairs           -> QUAL_PAIRS
+// QUAL_PAIRS holds only while ov_pairs, its count d_misc[MISC_OVERLAP] and the descriptors are those of the stage that
+// ran the tweak: nothing but launch_overlap writes the first two, and only a stage of the same batch (same n, so no
+// buffer moves) has run since.
+enum QualState : int {
+    QUAL_DIRTY,      // unknown or widely edited: the first stage after an upload, BAQ, -6, a stage that stopped early
+    QUAL_PAIRS,      // only k_overlap_tweak wrote, to the mates ov_pairs lists
+    QUAL_PRISTINE,   // equal to qual0
+};
+
 struct b200_engine {
     int device = 0, n_sm = 0;
     cudaStream_t stream = nullptr;
@@ -33,6 +48,7 @@ struct b200_engine {
     DBUF(uint32_t, cigar); DBUF(uint8_t, seq4); DBUF(uint8_t, qual); DBUF(char, ref); DBUF(char, dname);
     DBUF(int64_t, file_start);
     DBUF(uint8_t, qual0); DBUF(uint8_t, mapq0);   // pristine copies for b200_restage (b200_set_keep_raw)
+    QualState qual_state = QUAL_DIRTY;            // of qual against qual0 (keep_raw only)
     // derived
     DBUF(uint8_t, state); DBUF(int32_t, rlen); DBUF(plp::ReadDesc, desc); DBUF(int32_t, endv); DBUF(int32_t, pmax);
     DBUF(int32_t, glo); DBUF(int32_t, ghi); DBUF(uint64_t, status); DBUF(char, out);   // status: look-back state of the scans (scan.cuh)
@@ -93,7 +109,7 @@ enum : int {
     MISC_ENT2_CURSOR = 3,  // k_mp_entries: cursor of the second entry array
     MISC_COVERAGE = 8,     // 5 words: k_coverage's sums; read by b200_coverage
     MISC_BAQ = 16,         // 16 words: k_baq_plan's counters (first 5, read by launch_baq) and k_baq's work counter (word 11)
-    MISC_OVERLAP = 40,     // k_overlap: number of pairs to tweak; read by k_overlap_tweak
+    MISC_OVERLAP = 40,     // k_overlap: number of pairs to tweak; read by k_overlap_tweak and, at the next restage, k_qual_restore
     MISC_QSUM_DEEP = 41,   // k_mp_qsums / k_ind_qsums: a column or allele too deep for 32-bit sums; read by their calls
     MISC_PSUM_OVF = 42,    // k_mp_psums / k_ind_psums: a sum of squared read positions past INT64_MAX; read by their calls
     MISC_RANK_DEEP = 43,   // k_rank_counts: a column with more class entries than exact rank sums allow; read by b200_mpileup_ranksums
@@ -103,4 +119,5 @@ using plp::RawSoA;
 int build_ranges(b200_engine *e, int *max_range);
 int launch_baq(b200_engine *e, const RawSoA &r, const b200_stage_conf_t &cf);
 int launch_overlap(b200_engine *e, const RawSoA &r);
+int launch_qual_restore(b200_engine *e, const RawSoA &r);
 int launch_depth_clip(b200_engine *e, const RawSoA &r);
